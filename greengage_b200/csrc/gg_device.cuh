@@ -22,6 +22,7 @@
 #include "gg_program.h"
 
 #define GG_FULL_MASK 0xffffffffu
+#define GG_F8_NEGZERO_BITS 0x8000000000000000ull    /* -0.0: where float8 sums start */
 
 namespace ggd {
 

@@ -27,7 +27,8 @@ gg_hashagg_kernel(const __grid_constant__ ggp_program P, const ScanAggParams prm
 	scanagg_body<MODE_HASH, DynPlan>(P, prm);
 }
 
-/* MIN/MAX start from the identity of their comparison; everything else from zero (the table is memset first) */
+/* MIN/MAX start from the identity of their comparison, float8 sums from -0 (RegAcc::zero); everything else from zero (the
+ * table is memset first) */
 __global__ void gg_hashagg_init_kernel(HashAggTable ha)
 {
 	for (int j = 0; j < ha.nacc; j++)
@@ -38,6 +39,7 @@ __global__ void gg_hashagg_init_kernel(HashAggTable ha)
 		else if (kind == GGP_ACC_F8MAX) init = 0xfff0000000000000ull;         /* -Infinity */
 		else if (kind == GGP_ACC_I8MIN) init = 0x7fffffffffffffffull;
 		else if (kind == GGP_ACC_I8MAX) init = 0x8000000000000000ull;
+		else if (kind == GGP_ACC_F8SUM) init = GG_F8_NEGZERO_BITS;
 		else continue;
 		for (uint64_t i = blockIdx.x * (uint64_t) blockDim.x + threadIdx.x; i < ha.cap; i += (uint64_t) gridDim.x * blockDim.x)
 			ha.ent[i * ha.stride + ha.off_acc + j] = init;
@@ -194,7 +196,7 @@ gg_merge_recs_kernel(const ggp_grec *recs, int nrecs, int nkeys, int nacc, ggp_a
 	{
 		int mg = t / V, j = t % V;
 		int kind = nacc > 0 ? kinds.k[j] : GGP_ACC_COUNT;
-		double s0 = 0.0, s1 = 0.0;
+		double s0 = kind == GGP_ACC_F8SUM ? -0.0 : 0.0, s1 = 0.0;
 		unsigned long long cnt = 0, nn = 0;
 		for (int set = lane; set < nsets; set += 32)
 		for (int slot = 0; slot < GGP_FAST_GROUPS; slot++)
@@ -975,12 +977,13 @@ static void finalize_rows(const gg_agg *agg, const ggp_aggmap *aggmap, const ggp
 				case GG_AGG_AVG_FLOAT8:
 					if (partial)
 					{
-						v.f[0] = (double) nn; v.f[1] = x.sum[col]; v.f[2] = x.sumsq[col];
+						/* float8_accum's state starts from "{0,0,0}": + 0.0 turns the -0 the sums start from into +0 */
+						v.f[0] = (double) nn; v.f[1] = x.sum[col] + 0.0; v.f[2] = x.sumsq[col] + 0.0;
 					}
 					else if (nn == 0)
 						v.isnull = 1;            /* float8_avg: N == 0 => NULL (float.c:1995) */
 					else
-						v.f[0] = x.sum[col] / (double) nn;
+						v.f[0] = (x.sum[col] + 0.0) / (double) nn;
 					break;
 				default:                      /* int sum/min/max */
 					v.isnull = nn == 0;

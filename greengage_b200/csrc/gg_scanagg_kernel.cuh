@@ -50,9 +50,11 @@ struct RegAcc {
 #define GG_RQ_DECL(G, J) double r##G##J;
 	GG_RQ_FOREACH(GG_RQ_DECL)
 #undef GG_RQ_DECL
+	/* float8 sums start from -0, the identity of IEEE addition: a sum is -0 exactly when every input was -0, as
+	 * float8pl's NULL initcond gives (the first input taken as it is) */
 	__device__ __forceinline__ void zero()
 	{
-#define GG_RQ_ZERO(G, J) r##G##J = 0.0;
+#define GG_RQ_ZERO(G, J) r##G##J = -0.0;
 		GG_RQ_FOREACH(GG_RQ_ZERO)
 #undef GG_RQ_ZERO
 	}
@@ -799,12 +801,13 @@ __device__ __forceinline__ void scanagg_body(const ggp_program &P, const ScanAgg
 	}
 	if (MODE == MODE_PRIV && warp < ncons)
 	{
-		/* zero this thread's private accumulators */
+		/* zero this thread's private accumulators: integer sums 0, float8 sums -0 (RegAcc::zero) */
 		for (int g = 0; g < gcap; g++)
 		{
 			sts32(smem_base + prm.cnt_off + (uint32_t) (g * NT + (int) threadIdx.x) * 4, 0);
 			for (int s = 0; s < nsl; s++)
-				sts64(smem_base + prm.acc_off + (uint32_t) ((g * nsl + s) * NT + (int) threadIdx.x) * 8, 0);
+				sts64(smem_base + prm.acc_off + (uint32_t) ((g * nsl + s) * NT + (int) threadIdx.x) * 8,
+				      ((PL::intmask(P) >> s) & 1) ? 0ull : GG_F8_NEGZERO_BITS);
 		}
 	}
 	__syncthreads();
@@ -844,7 +847,7 @@ __device__ __forceinline__ void scanagg_body(const ggp_program &P, const ScanAgg
 			pair_g[r] = p / V;
 			pair_j[r] = p % V;
 			pair_kind[r] = nacc == 0 ? GGP_ACC_COUNT : (pair_j[r] < nacc ? P.acckind[pair_j[r]] : GGP_ACC_F8SUM);
-			acc_sum[r] = 0.0; acc_cnt[r] = 0; acc_n[r] = 0;
+			acc_sum[r] = pair_kind[r] == GGP_ACC_F8SUM ? -0.0 : 0.0; acc_cnt[r] = 0; acc_n[r] = 0;
 		}
 	}
 	uint32_t err = 0;
@@ -1425,7 +1428,7 @@ __device__ __forceinline__ void scanagg_body(const ggp_program &P, const ScanAgg
 		{
 			const int g = e / V, sl = e % V;
 			const bool isint = ((PL::intmask(P) >> sl) & 1) != 0;
-			double s0 = 0.0;
+			double s0 = isint ? 0.0 : -0.0;
 			unsigned long long cnt = 0;
 			for (int t = lane; t < NT; t += 32)
 			{
@@ -1491,7 +1494,7 @@ __device__ __forceinline__ void scanagg_body(const ggp_program &P, const ScanAgg
 		int g = p / V, sl = p % V;
 		if (g >= G || g >= GGP_FAST_GROUPS) continue;
 		int kind = nacc == 0 ? GGP_ACC_COUNT : (sl < nacc ? P.acckind[sl] : GGP_ACC_F8SUM);
-		double s0 = 0.0;
+		double s0 = kind == GGP_ACC_F8SUM ? -0.0 : 0.0;
 		unsigned long long cnt = 0, nn = 0;
 		for (int w = 0; w < ncons; w++)
 		{

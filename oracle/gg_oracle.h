@@ -171,6 +171,30 @@ int or_seqscan_agg_mt(const gg_scan *scan, const gg_agg *partial, const gg_agg *
 
 const char *or_strerror(int code);
 
+/* ---------------- exact mode (checker only; or_agg.c) ----------------
+ * Off by default.  When on, every hash/plain Agg of a NORMAL or PARTIAL stage keeps, beside its normal state, the exact
+ * record of the float8 inputs of each aggregate: the exact sum, sum of absolute values and sum of fl(x*x) as fixed-point
+ * integers in units of 2^-1074 (the least subnormal), so any double adds exactly.  or_aggtable_emit writes one or_exact per
+ * (emitted row, aggregate), in its row order; or_exact_fetch copies them out.  The limbs are 32-bit two's-complement
+ * digits, least significant first, carries resolved at emit.  Single-threaded operators only: the record is global. */
+#define OR_XLIMBS            68      /* 2^-1074 .. 2^1024, times up to 2^31 inputs, and a sign */
+#define OR_XF_NAN            0x01
+#define OR_XF_PINF           0x02
+#define OR_XF_NINF           0x04
+#define OR_XF_ALL_NEGZERO    0x08    /* n > 0 and every input was -0 */
+#define OR_XF_POSZERO        0x10    /* some input was +0 */
+#define OR_XF_NEGZERO        0x20    /* some input was -0 */
+typedef struct or_exact {
+	int64_t  n;                      /* non-NULL inputs */
+	int32_t  flags;                  /* OR_XF_* */
+	int32_t  lowbit;                 /* exponent of the lowest set bit over the finite nonzero inputs (INT32_MAX: none) */
+	int32_t  lowbit_sq;              /* the same over the finite nonzero fl(x*x) */
+	int32_t  pad;
+	int64_t  sum[OR_XLIMBS], abs[OR_XLIMBS], sq[OR_XLIMBS];
+} or_exact;
+void or_exact_mode(int on);
+long or_exact_fetch(or_exact *out, long cap);     /* returns how many the last emit wrote */
+
 #ifdef __cplusplus
 }
 #endif

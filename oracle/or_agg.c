@@ -48,6 +48,7 @@ typedef struct or_entry {				/* HashAggEntry, execHHashagg.h:41 */
 	int32_t  keylen[GG_MAX_KEYS];
 	int32_t  keyisnull[GG_MAX_KEYS];
 	or_aggstate st[GG_MAX_AGGS];
+	or_exact *x[GG_MAX_AGGS];			/* exact mode: one per float8 aggregate, NULL otherwise */
 } or_entry;
 
 struct or_aggtable {
@@ -65,6 +66,9 @@ struct or_aggtable {
 	int nstreamed, capstreamed;
 	/* plain aggregation (numCols == 0): exactly one group, even on empty input (nodeAgg.c:1247-1400) */
 	or_entry *plain;
+	/* exact mode: whether this table keeps the records, and those of the streamed rows (nfloat per row) */
+	int exact, nfloat;
+	or_exact *streamed_x;
 };
 
 double
@@ -77,6 +81,152 @@ or_now(void)
 }
 
 static inline double as_f8(int64_t v) { double d; memcpy(&d, &v, 8); return d; }
+
+/* ---- exact mode (gg_oracle.h): what any order of summation must be measured against ---- */
+
+static int exact_on;
+static or_exact *exact_out;
+static long exact_nout, exact_cap;
+
+void
+or_exact_mode(int on)
+{
+	exact_on = on;
+}
+
+long
+or_exact_fetch(or_exact *out, long cap)
+{
+	long n = exact_nout < cap ? exact_nout : cap;
+
+	memcpy(out, exact_out, (size_t) n * sizeof *out);
+	return exact_nout;
+}
+
+static int
+is_f8_agg(int aggfnoid)
+{
+	return aggfnoid == GG_AGG_SUM_FLOAT8 || aggfnoid == GG_AGG_AVG_FLOAT8 ||
+		aggfnoid == GG_AGG_MIN_FLOAT8 || aggfnoid == GG_AGG_MAX_FLOAT8;
+}
+
+static void
+exact_init(or_exact *x)
+{
+	memset(x, 0, sizeof *x);
+	x->lowbit = x->lowbit_sq = INT32_MAX;
+}
+
+/* finite x = m * 2^e with integer m, e >= -1074: add sign*m at bit e + 1074 of the fixed-point limbs */
+static void
+limbs_add(int64_t *limb, double x, int *lowbit)
+{
+	int e, k, sh;
+	uint64_t m;
+	unsigned __int128 w;
+	double f;
+
+	if (x == 0.0)
+		return;
+	f = frexp(fabs(x), &e);				/* |x| = f * 2^e, f in [0.5, 1) */
+	if (e - 53 >= -1074)
+	{
+		m = (uint64_t) ldexp(f, 53);
+		e -= 53;
+	}
+	else
+	{
+		m = (uint64_t) ldexp(f, e + 1074);	/* subnormal */
+		e = -1074;
+	}
+	if (lowbit && e + __builtin_ctzll(m) < *lowbit)
+		*lowbit = e + __builtin_ctzll(m);
+	sh = e + 1074;
+	k = sh >> 5;
+	w = (unsigned __int128) m << (sh & 31);
+	for (; w != 0; k++, w >>= 32)
+		limb[k] += x < 0 ? -(int64_t) (uint32_t) w : (int64_t) (uint32_t) w;
+}
+
+static void
+exact_add(int aggfnoid, or_exact *x, double v)
+{
+	x->n++;
+	if (x->n == 1)
+		x->flags |= OR_XF_ALL_NEGZERO;
+	if (!(v == 0.0 && signbit(v)))
+		x->flags &= ~OR_XF_ALL_NEGZERO;
+	if (v == 0.0)
+		x->flags |= signbit(v) ? OR_XF_NEGZERO : OR_XF_POSZERO;
+	if (isnan(v))
+		x->flags |= OR_XF_NAN;
+	else if (isinf(v))
+		x->flags |= v > 0 ? OR_XF_PINF : OR_XF_NINF;
+	if (!isfinite(v) || aggfnoid == GG_AGG_MIN_FLOAT8 || aggfnoid == GG_AGG_MAX_FLOAT8)
+		return;
+	limbs_add(x->sum, v, &x->lowbit);
+	limbs_add(x->abs, fabs(v), NULL);
+	if (isfinite(v * v))
+		limbs_add(x->sq, v * v, &x->lowbit_sq);
+}
+
+/* carries into 32-bit digits; the top limb keeps the sign */
+static void
+limbs_normalise(int64_t *limb)
+{
+	int k;
+
+	for (k = 0; k < OR_XLIMBS - 1; k++)
+	{
+		int64_t c = limb[k] >> 32;			/* arithmetic shift: floor division by 2^32 */
+
+		limb[k] -= c * ((int64_t) 1 << 32);
+		limb[k + 1] += c;
+	}
+}
+
+static void
+exact_emit(const or_exact *x)
+{
+	or_exact *o;
+
+	if (exact_nout == exact_cap)
+	{
+		exact_cap = exact_cap ? exact_cap * 2 : 64;
+		exact_out = realloc(exact_out, (size_t) exact_cap * sizeof *exact_out);
+	}
+	o = &exact_out[exact_nout++];
+	if (x == NULL)
+		exact_init(o);
+	else
+		*o = *x;
+	limbs_normalise(o->sum);
+	limbs_normalise(o->abs);
+	limbs_normalise(o->sq);
+}
+
+static void
+entry_exact_init(const or_aggtable *t, or_entry *e)
+{
+	int i;
+
+	for (i = 0; t->exact && i < t->agg->numAggs; i++)
+		if (is_f8_agg(t->agg->aggs[i].aggfnoid))
+		{
+			e->x[i] = malloc(sizeof(or_exact));
+			exact_init(e->x[i]);
+		}
+}
+
+static void
+entry_free(or_entry *e)
+{
+	int i;
+
+	for (i = 0; i < GG_MAX_AGGS; i++)
+		free(e->x[i]);
+	free(e);
+}
 
 /* ---- transition machinery ---- */
 
@@ -398,6 +548,9 @@ or_aggtable_create(const gg_agg *agg, const gg_exprpool *pool, long max_entries)
 	t->buckets = calloc(t->nbuckets, sizeof *t->buckets);
 	t->bloom = calloc(t->nbuckets, sizeof *t->bloom);
 	t->max_entries = max_entries;
+	t->exact = exact_on && agg->aggstage != GG_AGGSTAGE_FINAL;
+	for (i = 0; i < agg->numAggs; i++)
+		t->nfloat += is_f8_agg(agg->aggs[i].aggfnoid);
 	for (i = 0; i < agg->numCols; i++)
 		t->keytype[i] = pool ? pool->nodes[agg->grpCol[i]].rettype : 0;
 	return t;
@@ -416,7 +569,7 @@ free_entries(or_aggtable *t)
 		{
 			or_entry *n = e->next;
 
-			free(e);
+			entry_free(e);
 			e = n;
 		}
 		t->buckets[b] = NULL;
@@ -431,7 +584,9 @@ or_aggtable_free(or_aggtable *t)
 	if (!t)
 		return;
 	free_entries(t);
-	free(t->plain);
+	if (t->plain)
+		entry_free(t->plain);
+	free(t->streamed_x);
 	free(t->buckets);
 	free(t->bloom);
 	free(t->streamed);
@@ -582,11 +737,18 @@ stream_out(or_aggtable *t)
 
 		for (e = t->buckets[b]; e; e = e->next)
 		{
+			int i, f = 0;
+
 			if (t->nstreamed == t->capstreamed)
 			{
 				t->capstreamed = t->capstreamed ? t->capstreamed * 2 : 64;
 				t->streamed = realloc(t->streamed, (size_t) t->capstreamed * sizeof(gg_aggrow));
+				if (t->exact)
+					t->streamed_x = realloc(t->streamed_x, (size_t) t->capstreamed * t->nfloat * sizeof(or_exact));
 			}
+			for (i = 0; t->exact && i < t->agg->numAggs; i++)
+				if (e->x[i])
+					t->streamed_x[(size_t) t->nstreamed * t->nfloat + f++] = *e->x[i];
 			row_from_entry(t, e, &t->streamed[t->nstreamed++]);
 		}
 	}
@@ -619,6 +781,7 @@ lookup(or_aggtable *t, uint32_t hashkey, const int64_t *key, const int32_t *keyl
 		entry->keylen[i] = keylen[i];
 		entry->keyisnull[i] = keyisnull[i];
 	}
+	entry_exact_init(t, entry);
 	for (i = 0; i < t->agg->numAggs; i++)
 	{
 		if (final_stage)
@@ -647,6 +810,7 @@ plain_entry(or_aggtable *t, int final_stage)
 	if (!t->plain)
 	{
 		t->plain = calloc(1, sizeof(or_entry));
+		entry_exact_init(t, t->plain);
 		for (i = 0; i < t->agg->numAggs; i++)
 		{
 			if (final_stage)
@@ -693,6 +857,8 @@ or_aggtable_advance(or_aggtable *t, or_row *outer, or_row *inner)
 			return rc;
 		if ((rc = advance_trans(ar->aggfnoid, &e->st[i], &arg)) != 0)
 			return rc;
+		if (e->x[i] && !arg.isnull)
+			exact_add(ar->aggfnoid, e->x[i], as_f8(arg.v));
 	}
 	return 0;
 }
@@ -701,19 +867,28 @@ int
 or_aggtable_emit(or_aggtable *t, gg_aggrow *out, int outcap, int *nout)
 {
 	unsigned b;
-	int n = 0, i;
+	int n = 0, i, j;
 
+	if (t->exact)
+		exact_nout = 0;
 	for (i = 0; i < t->nstreamed; i++)
 	{
 		if (n >= outcap)
 			return OR_ERR_NOMEM;
 		out[n++] = t->streamed[i];
+		for (j = 0; t->exact && j < t->nfloat; j++)
+			exact_emit(&t->streamed_x[(size_t) i * t->nfloat + j]);
 	}
 	if (t->agg->numCols == 0)
 	{
+		or_entry *e = plain_entry(t, t->agg->aggstage == GG_AGGSTAGE_FINAL);
+
 		if (n >= outcap)
 			return OR_ERR_NOMEM;
-		row_from_entry(t, plain_entry(t, t->agg->aggstage == GG_AGGSTAGE_FINAL), &out[n++]);
+		row_from_entry(t, e, &out[n++]);
+		for (j = 0; t->exact && j < t->agg->numAggs; j++)
+			if (e->x[j])
+				exact_emit(e->x[j]);
 	}
 	for (b = 0; b < t->nbuckets; b++)
 	{
@@ -724,6 +899,9 @@ or_aggtable_emit(or_aggtable *t, gg_aggrow *out, int outcap, int *nout)
 			if (n >= outcap)
 				return OR_ERR_NOMEM;
 			row_from_entry(t, e, &out[n++]);
+			for (j = 0; t->exact && j < t->agg->numAggs; j++)
+				if (e->x[j])
+					exact_emit(e->x[j]);
 		}
 	}
 	*nout = n;

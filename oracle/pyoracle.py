@@ -22,6 +22,57 @@ class or_datum(C.Structure):
                 ("hi", C.c_int64), ("dscale", C.c_int32), ("pad", C.c_int32)]
 
 
+XLIMBS = 68                     # OR_XLIMBS (gg_oracle.h)
+EXACT_SCALE = 1074              # the exact sums are integers in units of 2^-EXACT_SCALE
+XF_NAN, XF_PINF, XF_NINF, XF_ALL_NEGZERO, XF_POSZERO, XF_NEGZERO = 0x01, 0x02, 0x04, 0x08, 0x10, 0x20
+
+
+class or_exact(C.Structure):
+    _fields_ = [("n", C.c_int64), ("flags", C.c_int32), ("lowbit", C.c_int32), ("lowbit_sq", C.c_int32), ("pad", C.c_int32),
+                ("sum", C.c_int64 * XLIMBS), ("abs", C.c_int64 * XLIMBS), ("sq", C.c_int64 * XLIMBS)]
+
+
+class Exact:
+    """What the float8 inputs of one aggregate in one group were, exactly (the oracle's exact mode, or_agg.c).
+    s, a, q: the exact sum, sum of |x| and sum of fl(x*x) of the finite inputs, as integers in units of 2^-EXACT_SCALE;
+    lowbit (lowbit_sq): exponent of the lowest set bit over the nonzero inputs (squares), None when there are none."""
+    __slots__ = ("n", "flags", "lowbit", "lowbit_sq", "s", "a", "q")
+
+    def __init__(self, r):
+        self.n, self.flags = r.n, r.flags
+        self.lowbit = None if r.lowbit == 0x7FFFFFFF else r.lowbit
+        self.lowbit_sq = None if r.lowbit_sq == 0x7FFFFFFF else r.lowbit_sq
+        self.s, self.a, self.q = (int.from_bytes(np.ctypeslib.as_array(getattr(r, f)).astype(np.uint32).tobytes(), "little", signed=True)
+                                  for f in ("sum", "abs", "sq"))
+
+
+def _exact_states(agg, nrows):
+    """-> one list per emitted row: an Exact per aggregate (None for the non-float8 ones), in or_aggtable_emit's order"""
+    f8 = {capi.AGG_SUM_FLOAT8, capi.AGG_AVG_FLOAT8, capi.AGG_MIN_FLOAT8, capi.AGG_MAX_FLOAT8}
+    which = [agg.aggs[i].aggfnoid in f8 for i in range(agg.numAggs)]
+    nf = sum(which)
+    buf = (or_exact * max(nrows * nf, 1))()
+    got = lib().or_exact_fetch(buf, nrows * nf)
+    assert got == nrows * nf, (got, nrows, nf)
+    out, k = [], 0
+    for _ in range(nrows):
+        row = []
+        for w in which:
+            row.append(Exact(buf[k]) if w else None)
+            k += w
+        out.append(row)
+    return out
+
+
+class exact_mode:
+    """with po.exact_mode(): the operators record the exact inputs of every float8 aggregate (or_exact_mode)"""
+    def __enter__(self):
+        lib().or_exact_mode(1)
+
+    def __exit__(self, *a):
+        lib().or_exact_mode(0)
+
+
 def build():
     subprocess.check_call(["make", "-s", "-C", _HERE])
     if os.path.isdir("/root/reference/src"):
@@ -96,6 +147,10 @@ def lib():
                                           C.POINTER(vp), C.POINTER(i64), i32, i64, C.POINTER(capi.gg_aggrow), i32,
                                           C.POINTER(i32), C.POINTER(u64), C.POINTER(u64)]
         L.or_bctruelen.argtypes = [C.c_char_p, i32]
+        L.or_exact_mode.argtypes = [i32]
+        L.or_exact_mode.restype = None
+        L.or_exact_fetch.argtypes = [C.POINTER(or_exact), C.c_long]
+        L.or_exact_fetch.restype = C.c_long
         L.or_strerror.restype = C.c_char_p
         L.or_strerror.argtypes = [i32]
         _lib = L
@@ -179,6 +234,11 @@ def _chk(rc):
         raise OracleError(rc)
 
 
+def _exact(on):
+    import contextlib
+    return exact_mode() if on else contextlib.nullcontext()
+
+
 def _ptr(a):
     return a.ctypes.data_as(C.c_void_p)
 
@@ -236,14 +296,17 @@ def build_pages(desc, rows, nulls=None, all_visible=True):
 
 # ---- operators ----
 
-def seqscan_agg(scan, agg, pool, pages, cap=4096):
+def seqscan_agg(scan, agg, pool, pages, cap=4096, exact=False):
+    """-> (rows, scanned, passed); exact=True: (rows, scanned, passed, [Exact per aggregate] per row)"""
     nb = pages.size // capi.GG_BLCKSZ
     out = (capi.gg_aggrow * cap)()
     n = C.c_int32(0)
     sc, ps = C.c_uint64(0), C.c_uint64(0)
-    _chk(lib().or_seqscan_agg(C.byref(scan), C.byref(agg), C.byref(pool), _ptr(pages), nb, out, cap,
-                              C.byref(n), C.byref(sc), C.byref(ps)))
-    return [out[i] for i in range(n.value)], sc.value, ps.value
+    with _exact(exact):
+        _chk(lib().or_seqscan_agg(C.byref(scan), C.byref(agg), C.byref(pool), _ptr(pages), nb, out, cap,
+                                  C.byref(n), C.byref(sc), C.byref(ps)))
+    rows = [out[i] for i in range(n.value)]
+    return (rows, sc.value, ps.value) + ((_exact_states(agg, n.value),) if exact else ())
 
 
 def agg_final(agg, rows, cap=4096):
@@ -267,14 +330,16 @@ def seqscan_agg_mt(scan, partial, final, pool, pages, nthreads, cap=4096):
     return [out[i] for i in range(n.value)], secs.value, rows.value
 
 
-def hashjoin_agg(outer, inner, hj, agg, pool, opages, ipages, cap=4096):
+def hashjoin_agg(outer, inner, hj, agg, pool, opages, ipages, cap=4096, exact=False):
+    """-> (rows, joined); exact=True: (rows, joined, [Exact per aggregate] per row)"""
     out = (capi.gg_aggrow * cap)()
     n = C.c_int32(0)
     nj = C.c_uint64(0)
-    _chk(lib().or_hashjoin_agg(C.byref(outer), C.byref(inner), C.byref(hj), C.byref(agg), C.byref(pool),
-                               _ptr(opages), opages.size // capi.GG_BLCKSZ, _ptr(ipages), ipages.size // capi.GG_BLCKSZ,
-                               out, cap, C.byref(n), C.byref(nj)))
-    return [out[i] for i in range(n.value)], nj.value
+    with _exact(exact):
+        _chk(lib().or_hashjoin_agg(C.byref(outer), C.byref(inner), C.byref(hj), C.byref(agg), C.byref(pool),
+                                   _ptr(opages), opages.size // capi.GG_BLCKSZ, _ptr(ipages), ipages.size // capi.GG_BLCKSZ,
+                                   out, cap, C.byref(n), C.byref(nj)))
+    return ([out[i] for i in range(n.value)], nj.value) + ((_exact_states(agg, n.value),) if exact else ())
 
 
 def hashjoin_tids(outer, inner, hj, pool, opages, ipages, cap=1 << 22):
@@ -406,17 +471,20 @@ def aocs_read_column(att, file, nrows_cap, checksum=True, ref=False):
     return vals[:n], nl[:n], fr[:nb.value], rc[:nb.value]
 
 
-def aocs_seqscan_agg(scan, agg, pool, colfiles, nrows, checksum=True, cap=4096):
-    """colfiles: one uint8 array per attribute of scan.desc, None for columns the plan does not read"""
+def aocs_seqscan_agg(scan, agg, pool, colfiles, nrows, checksum=True, cap=4096, exact=False):
+    """colfiles: one uint8 array per attribute of scan.desc, None for columns the plan does not read.
+    -> (rows, scanned, passed); exact=True: (rows, scanned, passed, [Exact per aggregate] per row)"""
     natts = scan.desc.natts
     ptrs = (C.c_void_p * natts)(*[None if f is None else f.ctypes.data for f in colfiles])
     sizes = (C.c_int64 * natts)(*[0 if f is None else f.size for f in colfiles])
     out = (capi.gg_aggrow * cap)()
     n = C.c_int32(0)
     sc, ps = C.c_uint64(0), C.c_uint64(0)
-    _chk(lib().or_aocs_seqscan_agg(C.byref(scan), C.byref(agg), C.byref(pool), ptrs, sizes, int(checksum), nrows, out, cap,
-                                   C.byref(n), C.byref(sc), C.byref(ps)))
-    return [out[i] for i in range(n.value)], sc.value, ps.value
+    with _exact(exact):
+        _chk(lib().or_aocs_seqscan_agg(C.byref(scan), C.byref(agg), C.byref(pool), ptrs, sizes, int(checksum), nrows, out, cap,
+                                       C.byref(n), C.byref(sc), C.byref(ps)))
+    rows = [out[i] for i in range(n.value)]
+    return (rows, sc.value, ps.value) + ((_exact_states(agg, n.value),) if exact else ())
 
 
 _snapshot_keep = None

@@ -3,6 +3,7 @@ import ctypes as C
 import json
 import os
 import struct
+from fractions import Fraction
 
 import numpy as np
 
@@ -120,11 +121,100 @@ def rows_by_key(rows, nkeys=2):
     return out
 
 
-def assert_aggrows_match(got, want, agg, rel=1e-6, float_exact=False):
-    """Integer results and keys bit-exact; float8 sums/avgs within `rel` (the tolerance BASELINE.json states)."""
+def exact_by_key(rows, states, nkeys):
+    """the oracle's exact records (po.seqscan_agg(..., exact=True)[-1]) keyed like rows_by_key, for comparing another
+    stage's rows (a FINAL over the same inputs) with them"""
+    return {k: states[i] for i, k in enumerate(rows_by_key(rows, nkeys))}
+
+
+_U = Fraction(1, 1 << 53)                  # unit roundoff of binary64
+
+
+def _gamma(k):
+    """γ(k) = k·u / (1 - k·u): |fl(Σ) - Σ| <= γ(n-1)·Σ|x| for any summation tree over n values (Higham, ASNA §4.2)"""
+    return k * _U / (1 - k * _U)
+
+
+def _exact_regime(total_abs, lowbit):
+    """every partial sum of every order is representable: all inputs are multiples of g = 2^lowbit and Σ|x| < 2^53·g"""
+    return lowbit is None or total_abs < (1 << (53 + lowbit + po.EXACT_SCALE))
+
+
+def _check_exact_sum(x, n, s, a, lowbit, nan, pinf, ninf, zero, ctx):
+    """one float8 sum `x` of n inputs against their exact sum s and Σ|x| a (integers in units of 2^-EXACT_SCALE).
+    zero: the float a zero sum must be (its sign)"""
+    if nan or (pinf and ninf):
+        assert x != x, ("NaN expected",) + ctx
+        return
+    if pinf or ninf:
+        assert x == (float("inf") if pinf else -float("inf")), ("infinity expected", x) + ctx
+        return
+    scale = 1 << po.EXACT_SCALE
+    if _exact_regime(a, lowbit):
+        want = zero if s == 0 else s / scale            # int / int: correctly rounded, and exact here
+        assert f2b(x) == f2b(want), ("not the exact sum", x, want) + ctx
+        return
+    assert abs(x) != float("inf") and x == x, ("finite sum expected", x) + ctx
+    err = abs(Fraction(x) - Fraction(s, scale))
+    bound = _gamma(n - 1) * Fraction(a, scale)
+    assert err <= bound, ("sum outside γ(n-1)·Σ|x|", x, float(Fraction(s, scale)), float(err), float(bound)) + ctx
+
+
+_OVERFLOW = Fraction((1 << 1024) - (1 << 970))        # sums at or past this round to infinity (DBL_MAX + half an ulp)
+
+
+def sum_overflow_rule(e, scale_exp=0):
+    """Whether float8pl's overflow ERROR is the same in every summation order of the finite inputs `e` records (an Exact of
+    values scaled by 2^-scale_exp): True every order overflows — all inputs share a sign and even the smallest sum any order
+    can compute, (1 - γ(n-1))·|s|, is past the overflow threshold; False no order does — the largest any order can compute,
+    (1 + γ(n-1))·Σ|x|, stays below it; None it depends on the order, and nothing may be asserted."""
+    scale = Fraction(1 << scale_exp, 1 << po.EXACT_SCALE)
+    s, a, g = abs(Fraction(e.s) * scale), Fraction(e.a) * scale, _gamma(e.n - 1)
+    if s == a and (1 - g) * s >= _OVERFLOW:
+        return True
+    if (1 + g) * a < _OVERFLOW:
+        return False
+    return None
+
+
+def _check_exact(fn, partial, j, x, e, ctx):
+    nan, pinf, ninf = bool(e.flags & po.XF_NAN), bool(e.flags & po.XF_PINF), bool(e.flags & po.XF_NINF)
+    if fn == capi.AGG_SUM_FLOAT8:
+        # float8pl with a NULL initcond takes the first input as it is: -0 exactly when every input was -0, in any order
+        _check_exact_sum(x, e.n, e.s, e.a, e.lowbit, nan, pinf, ninf, -0.0 if e.flags & po.XF_ALL_NEGZERO else 0.0, ctx)
+    elif partial and j == 1:                        # float8_accum's sumX starts from the +0 of "{0,0,0}"
+        _check_exact_sum(x, e.n, e.s, e.a, e.lowbit, nan, pinf, ninf, 0.0, ctx)
+    elif partial and j == 2:                        # sumX2 over fl(x*x) >= 0: an infinite input squares to +inf
+        _check_exact_sum(x, e.n, e.q, e.q, e.lowbit_sq, nan, pinf or ninf, False, 0.0, ctx)
+    else:                                           # float8_avg: sumX / N
+        if nan or pinf or ninf:
+            _check_exact_sum(x, e.n, e.s, e.a, e.lowbit, nan, pinf, ninf, 0.0, ctx)
+            return
+        scale = 1 << po.EXACT_SCALE
+        if _exact_regime(e.a, e.lowbit):
+            want = (e.s / scale + 0.0) / e.n            # the exact sum, then one correctly rounded division
+            assert f2b(x) == f2b(want), ("not fl(s/n)", x, want) + ctx
+            return
+        assert abs(x) != float("inf") and x == x, ("finite avg expected", x) + ctx
+        s, a, g = Fraction(e.s, scale), Fraction(e.a, scale), _gamma(e.n - 1)
+        err = abs(Fraction(x) - s / e.n)
+        bound = g * a / e.n + _U * (abs(s) + g * a) / e.n
+        assert err <= bound, ("avg outside its bound", x, float(s / e.n), float(err), float(bound)) + ctx
+
+
+def assert_aggrows_match(got, want, agg, rel=1e-6, float_exact=False, exact=None):
+    """Integer results and keys bit-exact; float8 sums/avgs within `rel` (the tolerance BASELINE.json states).
+
+    exact: the oracle's exact records of the same inputs (po.seqscan_agg / hashjoin_agg / aocs_seqscan_agg with exact=True:
+    a list aligned with `want`, or exact_by_key's dict).  Then every float8 SUM/AVG is held to what any summation order
+    provably gives instead of `rel`: bit for bit the exact answer where every partial sum is representable, else within
+    γ(n-1)·Σ|x| of the exact sum; NaN / ±inf as the non-finite inputs dictate."""
     nkeys = agg.numCols
     g, w = rows_by_key(got, nkeys), rows_by_key(want, nkeys)
     assert set(g) == set(w), (sorted(g), sorted(w))
+    if isinstance(exact, list):
+        exact = dict(zip(w, exact))
+    partial = agg.aggstage == capi.AGGSTAGE_PARTIAL
     for k in w:
         for i in range(agg.numAggs):
             a, b = g[k].agg[i], w[k].agg[i]
@@ -136,15 +226,111 @@ def assert_aggrows_match(got, want, agg, rel=1e-6, float_exact=False):
                       capi.AGG_MAX_INT8, capi.AGG_MIN_INT8, capi.AGG_MAX_DATE, capi.AGG_MIN_DATE):
                 assert a.i == b.i, (k, i, a.i, b.i)
             else:
-                nf = 3 if (fn == capi.AGG_AVG_FLOAT8 and agg.aggstage == capi.AGGSTAGE_PARTIAL) else 1
+                nf = 3 if (fn == capi.AGG_AVG_FLOAT8 and partial) else 1
+                e = exact[k][i] if exact is not None else None
                 for j in range(nf):
                     x, y = a.f[j], b.f[j]
-                    if fn in (capi.AGG_MAX_FLOAT8, capi.AGG_MIN_FLOAT8) or float_exact or (nf == 3 and j == 0):
+                    if fn in (capi.AGG_MAX_FLOAT8, capi.AGG_MIN_FLOAT8):
+                        if e is not None and x == 0 and y == 0 and e.flags & po.XF_POSZERO and e.flags & po.XF_NEGZERO:
+                            # float8larger/smaller keep the later argument of a tie, so with both zeros in the group the
+                            # reference's sign depends on scan order; a parallel scan has none, either sign is right
+                            continue
                         assert f2b(x) == f2b(y) or (x != x and y != y), (k, i, j, x, y)
+                    elif float_exact or (nf == 3 and j == 0):
+                        assert f2b(x) == f2b(y) or (x != x and y != y), (k, i, j, x, y)
+                    elif e is not None:
+                        _check_exact(fn, partial, j, x, e, (k, i, j))
                     elif y == 0 or y != y or abs(y) == float("inf"):
                         assert x == y or (x != x and y != y), (k, i, j, x, y)
                     else:
                         assert abs(x - y) <= rel * abs(y), (k, i, j, x, y)
+
+
+# ---- a relation built for the edges of float8 summation ----
+
+EDGE_GROUPS = {
+    0: "every input -0", 1: "+0 and -0 mixed", 2: "+inf alone", 3: "+inf with -inf", 4: "NaN among finite values",
+    5: "multiples of 2^-10, heavy cancellation, sum|x| just under 2^43 (exact in any order)",
+    6: "non-dyadic values that cancel: sum|x| >> |sum|", 7: "one input", 8: "31 inputs", 9: "32 inputs", 10: "33 inputs",
+    11: "2000 inputs laid out across a page boundary", 12: "every input NULL", 13: "-inf alone, with NULLs",
+    14: "zeros of both signs and negative values (min ties at neither zero)", 15: "-0 and positive values (min is -0)",
+}
+
+
+def edge_relation(nullable=True, pad=0):
+    """(desc, pages, nrows): (g int4, v float8) rows of the EDGE_GROUPS, seeded, most groups shuffled over ~10 pages;
+    NULL v is mixed into several groups.  nullable=False: the same rows without the NULL ones, v declared NOT NULL.
+    pad: that many float8 columns (all 0, never aggregated) after v, for tuples wide enough that a page holds fewer than
+    10 chunks of 32 rows — the shape on which the private-accumulator kernels keep sums in registers."""
+    if ("edge", nullable, pad) in _fixture_cache:
+        return _fixture_cache[("edge", nullable, pad)]
+    rng = np.random.default_rng(2024)
+    rows = []
+    rows += [(0, -0.0)] * 200
+    rows += [(1, z) for z in rng.choice([0.0, -0.0], 300)]
+    rows += [(2, float("inf"))]
+    rows += [(3, float("inf")), (3, -float("inf"))] + [(3, float(x)) for x in rng.normal(size=20)]
+    rows += [(4, float("nan"))] + [(4, float(x)) for x in rng.normal(size=60)]
+    n5 = 3000
+    half = rng.integers((1 << 53) // n5 // 2, (1 << 53) // n5 - 8, n5 // 2, dtype=np.int64) * rng.choice([-1, 1], n5 // 2)
+    k = np.concatenate([half, -half])                        # the total cancels but for the few units added here
+    k[0] += 3 if k[0] > 0 else -3
+    k[1] -= 1 if k[1] > 0 else -1
+    assert (1 << 52) < int(np.abs(k).sum()) < 1 << 53
+    rows += [(5, float(int(v)) * 2.0 ** -10) for v in k]
+    x6 = rng.normal(size=600) * 1e8
+    rows += [(6, float(v)) for v in np.concatenate([x6, -x6 * (1 + 1e-12), [0.1]])]
+    rows += [(7, 0.3)]
+    for gid, n in ((8, 31), (9, 32), (10, 33)):
+        rows += [(gid, float(v)) for v in rng.normal(size=n) / 3]
+    rows += [(14, v) for v in (0.0, -0.0, -1.5, 0.0, -2.25)]
+    rows += [(15, v) for v in (1.0, -0.0, 0.5)]
+    nulls = [False] * len(rows)
+    rows += [(12, 0.0)] * 7
+    nulls += [True] * 7
+    rows += [(13, -float("inf")), (13, 0.0), (13, 0.0)]
+    nulls += [False, True, True]
+    for gid in (1, 4, 5, 8):                                # NULLs mixed into groups that have values
+        rows += [(gid, 0.0)] * 5
+        nulls += [True] * 5
+    order = rng.permutation(len(rows))
+    rows, nulls = [rows[i] for i in order], [nulls[i] for i in order]
+    # group 11 kept contiguous in the middle of the relation, so that it straddles a page boundary
+    mid = len(rows) // 2
+    g11 = [(11, float(v)) for v in rng.normal(size=2000) * 7.25]
+    rows, nulls = rows[:mid] + g11 + rows[mid:], nulls[:mid] + [False] * len(g11) + nulls[mid:]
+    if not nullable:
+        rows, nulls = [r for r, isn in zip(rows, nulls) if not isn], [False] * (len(rows) - sum(nulls))
+    desc = make_desc([(capi.INT4OID, 4, "i", 1, 1), (capi.FLOAT8OID, 8, "d", 1, 0 if nullable else 1)] + [(capi.FLOAT8OID, 8, "d", 1, 1)] * pad)
+    pages = po.build_pages(desc, [list(r) + [0.0] * pad for r in rows], [[False, n] + [False] * pad for n in nulls])
+    _fixture_cache[("edge", nullable, pad)] = (desc, pages, len(rows))
+    return _fixture_cache[("edge", nullable, pad)]
+
+
+def edge_plan(desc, stage=capi.AGGSTAGE_NORMAL):
+    """GROUP BY g: count(*), sum(v), avg(v), min(v), max(v), count(v), sum(v * 0.5)"""
+    p = capi.ExprPool()
+    g, v = p.var(1, capi.INT4OID), p.var(2, capi.FLOAT8OID)
+    half = p.func(capi.F_FLOAT8MUL, capi.FLOAT8OID, v, p.const(capi.FLOAT8OID, 0.5))
+    agg = capi.make_agg(stage, [g], [(capi.AGG_COUNT_STAR, -1), (capi.AGG_SUM_FLOAT8, v), (capi.AGG_AVG_FLOAT8, v), (capi.AGG_MIN_FLOAT8, v),
+                                     (capi.AGG_MAX_FLOAT8, v), (capi.AGG_COUNT_ANY, v), (capi.AGG_SUM_FLOAT8, half)])
+    return capi.make_scan(desc, -1), agg, p.pool
+
+
+def edge_sum_plan(desc, groups, stage=capi.AGGSTAGE_NORMAL, num_groups=0):
+    """WHERE g IN (groups) GROUP BY g: sum(v), avg(v), sum(v * 0.5) — sums only, so that a NOT NULL v runs on the
+    private-accumulator kernels (which take no MIN/MAX); `groups` should leave out the non-finite ones, whose private sums
+    are replayed on the interpreter kernel"""
+    p = capi.ExprPool()
+    g, v = p.var(1, capi.INT4OID), p.var(2, capi.FLOAT8OID)
+    q = -1
+    for x in groups:
+        eq = p.func(capi.F_INT4EQ, capi.BOOLOID, g, p.const(capi.INT4OID, x))
+        q = eq if q < 0 else p.boolop(capi.E_OR, q, eq)
+    half = p.func(capi.F_FLOAT8MUL, capi.FLOAT8OID, v, p.const(capi.FLOAT8OID, 0.5))
+    agg = capi.make_agg(stage, [g], [(capi.AGG_SUM_FLOAT8, v), (capi.AGG_AVG_FLOAT8, v), (capi.AGG_SUM_FLOAT8, half), (capi.AGG_COUNT_STAR, -1)],
+                        num_groups=num_groups)
+    return capi.make_scan(desc, q), agg, p.pool
 
 
 # ---- the reference's regression lineitem / orders as join-shaped relations (tests/golden/*.npz) ----

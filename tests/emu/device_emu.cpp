@@ -55,6 +55,8 @@ struct HostSink {
 		{
 			EmuGroup g;
 			memset(&g, 0, sizeof g);
+			for (int j = 0; j < P->nacc; j++)                  /* float8 sums start from -0, as the kernels' accumulators do */
+				if (P->acckind[j] == GGP_ACC_F8SUM) g.sum[j] = -0.0;
 			for (int i = 0; i < GG_MAX_KEYS; i++) g.key[i] = id[i];
 			g.keynull = knull;
 			it = groups.emplace(id, g).first;

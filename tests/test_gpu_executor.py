@@ -1,10 +1,14 @@
 """The executor-node surface end to end on the GPU: plans are built the way the Postgres-side translator builds
 them, run through GgExecInitNode / GgExecProcNode / GgExecEndNode, and checked against the reference's golden Q1
-answer (ORDER BY included) and the oracle."""
+answer (ORDER BY included) and the oracle.  The golden answer is printed to fewer digits than a float8 holds, so it is
+met within 1e-6; float8 sums and averages are held to the oracle's exact record of the same pages
+(_util.assert_aggrows_match with exact=)."""
+import ctypes as C
+
 import numpy as np
 import pytest
 
-from _util import golden, lineitem_fixture_pages
+from _util import assert_aggrows_match, golden, lineitem_fixture_pages
 from greengage_b200 import capi, executor as ex, tpch
 from oracle import pyoracle as po
 
@@ -21,6 +25,42 @@ def eng():
 
 def b2f(v):
     return np.int64(v).view(np.float64).item()
+
+
+FLOAT_AGGS = (capi.AGG_SUM_FLOAT8, capi.AGG_AVG_FLOAT8, capi.AGG_MIN_FLOAT8, capi.AGG_MAX_FLOAT8)
+
+
+def as_aggrows(rows, want, agg, row_key, want_key):
+    """executor rows (grouping columns, then one column per aggregate) as gg_aggrows, keyed by the oracle row of the same
+    group so that assert_aggrows_match compares them; row_key(v, ln) and want_key(aggrow) name a group the same way"""
+    by = {want_key(w): w for w in want}
+    out = []
+    for v, nl, ty, ln in rows:
+        r = capi.gg_aggrow()
+        C.memmove(C.byref(r), C.byref(by[row_key(v, ln)]), C.sizeof(r))       # the keys, in the oracle's encoding
+        for i in range(agg.numAggs):
+            col = agg.numCols + i
+            r.agg[i].isnull = nl[col]
+            if agg.aggs[i].aggfnoid in FLOAT_AGGS:
+                r.agg[i].f[0] = b2f(v[col])
+            else:
+                r.agg[i].i = v[col]
+        out.append(r)
+    return out
+
+
+def q1_oracle(desc, pages, exp):
+    """(agg, oracle rows, exact record) of the one-stage Q1 over the pages: what a one- or two-stage plan must meet"""
+    scan, agg, pool = tpch.q1_plan(capi.TAB_LINEITEM_WIDE, capi.AGGSTAGE_NORMAL, interval_days=exp["interval_days"], desc=desc)
+    want, _, _, want_x = po.seqscan_agg(scan, agg, pool, pages, exact=True)
+    return agg, want, want_x
+
+
+def check_q1_exact(rows, oracle):
+    agg, want, want_x = oracle
+    key = lambda a, la, b, lb: (capi.unpack_str(a, la), capi.unpack_str(b, lb))
+    got = as_aggrows(rows, want, agg, lambda v, ln: key(v[0], ln[0], v[1], ln[1]), lambda w: key(w.key[0], w.keylen[0], w.key[1], w.keylen[1]))
+    assert_aggrows_match(got, want, agg, exact=want_x)
 
 
 def q1_sorted_plan(b, scan, agg, two_stage):
@@ -56,6 +96,7 @@ def test_q1_end_to_end_matches_the_reference_answer(eng, two_stage):
             for col, name in ((2, "sum_qty"), (3, "sum_base_price"), (4, "sum_disc_price"), (5, "sum_charge"),
                               (6, "avg_qty"), (7, "avg_price"), (8, "avg_disc")):
                 assert abs(b2f(v[col]) - float(w[name])) <= 1e-6 * abs(float(w[name])), (name, b2f(v[col]), w[name])
+        check_q1_exact(rows, q1_oracle(desc, pages, exp))           # two stages: one tree over the same inputs, same bound
         assert x.rows() == []                                       # end of stream stays end of stream
         x.rescan()
         assert len(x.rows()) == len(want)                           # ExecReScan runs the slice again
@@ -71,7 +112,7 @@ def test_join_through_the_node_surface(eng):
     li, _, _ = tpch.synth_generate(tpch.synth_spec(capi.TAB_LINEITEM_NARROW, 100_000, seed=6, norders=20_000))
     od, _, _ = tpch.synth_generate(tpch.synth_spec(capi.TAB_ORDERS, 15_000, seed=6))
     outer, inner, hj, agg, pool = tpch.join_plan(capi.TAB_LINEITEM_NARROW, "q3ish", capi.JOIN_INNER)
-    want, _ = po.hashjoin_agg(outer, inner, hj, agg, pool, li, od)
+    want, _, want_x = po.hashjoin_agg(outer, inner, hj, agg, pool, li, od, exact=True)
     lrel, orel = Relation(eng, host_pages=li), Relation(eng, host_pages=od)
     b = ex.PlanBuilder()
     plan = b.sort(b.agg(b.hashjoin(b.seqscan(0, outer.desc, outer.qual), b.hash(b.seqscan(1, inner.desc, inner.qual)), hj), agg),
@@ -81,11 +122,7 @@ def test_join_through_the_node_surface(eng):
         rows = x.rows()
         keys = [capi.unpack_str(v[0], ln[0]) for v, nl, ty, ln in rows]
         assert keys == sorted(keys, reverse=True) and len(rows) == len(want)
-        by = {r.key[0]: r for r in want}
-        for v, nl, ty, ln in rows:
-            w = by[v[0]]
-            assert v[1] == w.agg[0].i and v[3] == w.agg[2].i
-            assert abs(b2f(v[2]) - w.agg[1].f[0]) <= 1e-6 * abs(w.agg[1].f[0])
+        assert_aggrows_match(as_aggrows(rows, want, agg, lambda v, ln: v[0], lambda w: w.key[0]), want, agg, exact=want_x)
     finally:
         x.end()
         lrel.free()
@@ -114,7 +151,7 @@ def test_device_errors_surface_through_exec_proc_node(eng):
 
 # ---- results that stay on the device between the nodes of a slice (gg_groups / datum rows) and the C interconnect ----
 
-def _check_q1_rows(rows, exp):
+def _check_q1_rows(rows, exp, oracle):
     by = {(capi.unpack_str(v[0], ln[0]), capi.unpack_str(v[1], ln[1])): v for v, nl, ty, ln in rows}
     assert len(by) == len(rows) == len(exp["rows"])
     for w in exp["rows"]:
@@ -123,6 +160,7 @@ def _check_q1_rows(rows, exp):
         for col, name in ((2, "sum_qty"), (3, "sum_base_price"), (4, "sum_disc_price"), (5, "sum_charge"),
                           (6, "avg_qty"), (7, "avg_price"), (8, "avg_disc")):
             assert abs(b2f(v[col]) - float(w[name])) <= 1e-6 * abs(float(w[name])), (name, b2f(v[col]), w[name])
+    check_q1_exact(rows, oracle)
 
 
 def test_two_stage_q1_stays_on_the_device_through_the_interconnect(eng):
@@ -137,14 +175,15 @@ def test_two_stage_q1_stays_on_the_device_through_the_interconnect(eng):
     b = ex.PlanBuilder()
     plan, pool = tpch.q1_exec_plan(b, two_stage=True, interval_days=exp["interval_days"], desc=desc)
     x = ex.Executor(eng, pool, [rel], plan, interconnect=ic)
+    oracle = q1_oracle(desc, pages, exp)      # the device FINAL against the exact record of the one-stage scan of the pages
     try:
         rows = x.rows()
-        _check_q1_rows(rows, exp)
+        _check_q1_rows(rows, exp, oracle)
         loc = x.locations()
         assert [k for k, _ in loc] == ["motion", "aggfinal", "motion", "scanagg"]
         assert loc[1][1] == "device-groups" and loc[2][1] == "device-groups"      # FINAL Agg and Redistribute: no host rows
         x.rescan()
-        _check_q1_rows(x.rows(), exp)
+        _check_q1_rows(x.rows(), exp, oracle)
     finally:
         x.end()
         ic.close()
@@ -163,7 +202,7 @@ def test_scan_of_a_relation_in_host_memory(eng):
     plan, pool = tpch.q1_exec_plan(b, two_stage=False, interval_days=exp["interval_days"], desc=desc)
     x = ex.Executor(eng, pool, [(addr, pages.size // capi.GG_BLCKSZ)], plan)
     try:
-        _check_q1_rows(x.rows(), exp)
+        _check_q1_rows(x.rows(), exp, q1_oracle(desc, pages, exp))
     finally:
         x.end()
         host_free(addr)
@@ -179,7 +218,7 @@ def test_redistribute_hashjoin_plan(eng, kind, redistribute):
     li, _, _ = tpch.synth_generate(tpch.synth_spec(capi.TAB_LINEITEM_NARROW, 120_000, seed=9, norders=30_000))
     od, _, _ = tpch.synth_generate(tpch.synth_spec(capi.TAB_ORDERS, 25_000, seed=9))
     outer, inner, hj, agg, pool0 = tpch.join_plan(capi.TAB_LINEITEM_NARROW, kind, capi.JOIN_INNER)
-    want, nj = po.hashjoin_agg(outer, inner, hj, agg, pool0, li, od)
+    want, nj, want_x = po.hashjoin_agg(outer, inner, hj, agg, pool0, li, od, exact=True)
     lrel, orel = Relation(eng, host_pages=li), Relation(eng, host_pages=od)
     ic = Interconnect(eng, 1, 0)
     b = ex.PlanBuilder()
@@ -192,13 +231,10 @@ def test_redistribute_hashjoin_plan(eng, kind, redistribute):
             v = rows[0][0]
             w = want[0]
             assert v[0] == w.agg[0].i == nj and v[1] == w.agg[1].i               # count(*), sum(o_custkey): bit-exact
-            assert abs(b2f(v[2]) - w.agg[2].f[0]) <= 1e-6 * abs(w.agg[2].f[0])
+            got = as_aggrows(rows, want, agg, lambda v, ln: (), lambda w: ())
         else:
-            by = {r.key[0]: r for r in want}
-            for v, nl, ty, ln in rows:
-                w = by[v[0]]
-                assert v[1] == w.agg[0].i and v[3] == w.agg[2].i
-                assert abs(b2f(v[2]) - w.agg[1].f[0]) <= 1e-6 * abs(w.agg[1].f[0])
+            got = as_aggrows(rows, want, agg, lambda v, ln: v[0], lambda w: w.key[0])
+        assert_aggrows_match(got, want, agg, exact=want_x)
         if redistribute:
             L = ex.exec_lib()
             join_state = L.GgExecOuterPlanState(L.GgExecOuterPlanState(x.state))      # Agg(FINAL) -> Gather -> Agg over the join

@@ -46,7 +46,7 @@ def random_join_case(seed):
 @pytest.mark.parametrize("seed", list(range(20)))
 def test_random_join(eng, seed):
     outer, inner, hj, agg, p, opages, ipages, what = random_join_case(seed)
-    want, nj_want = po.hashjoin_agg(outer, inner, hj, agg, p.pool, opages, ipages, cap=20_000)
+    want, nj_want, want_x = po.hashjoin_agg(outer, inner, hj, agg, p.pool, opages, ipages, cap=20_000, exact=True)
     got, nj, _ = gpu_joinagg(eng, outer, inner, hj, agg, p.pool, opages, ipages, twice=(seed % 3 == 0))
     assert nj == nj_want, what
-    assert_aggrows_match(got, want, agg)
+    assert_aggrows_match(got, want, agg, exact=want_x)
