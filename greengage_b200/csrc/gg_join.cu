@@ -1,21 +1,13 @@
 /*
- * gg_join.cu — Hash / HashJoin (+ the Agg above): build and probe kernels (interpreter path) and the host pipeline
- * behind gg_joinagg_* (include/ggb200.h).  The probe side IS a gg_scanagg pipeline (gg_pipeline.h) whose row program
- * has a per-match piece; everything after the probe (merge, fetch, escalation to the general HashAggregate) is shared.
+ * gg_join.cu — Hash / HashJoin (+ the Agg above): the build kernel and the probe into the general HashAggregate (interpreter
+ * path), and the host pipeline behind gg_joinagg_* (include/ggb200.h).  The probe side IS a gg_scanagg pipeline (gg_pipeline.h)
+ * whose row program has a per-match piece; everything after the probe (merge, fetch, escalation to the general HashAggregate)
+ * is shared, and gg_scanagg.cu launches its kernels.
  */
 #include "gg_pipeline.h"
 #include "gg_groups.h"
 
 using namespace ggd;
-
-/* HashJoin probe side: the same scan front end; every outer row probes the join hash table and each
- * match runs the per-match piece of the program (join qual, grouping keys, aggregate arguments) */
-template <int MODE>
-__global__ void __launch_bounds__(MODE == MODE_PRIV ? 704 : 256, MODE == MODE_PRIV ? 1 : 2)
-gg_joinprobe_kernel(const __grid_constant__ ggp_program P, const ScanAggParams prm)
-{
-	scanagg_body<MODE, DynPlan, true>(P, prm);
-}
 
 /* Hash node: scan the inner relation into the join hash table */
 __global__ void __launch_bounds__(256, 2)
@@ -50,29 +42,6 @@ __global__ void gg_clear_matched_kernel(unsigned long long *ent, uint64_t slots,
 {
 	for (uint64_t i = blockIdx.x * (uint64_t) blockDim.x + threadIdx.x; i < slots; i += (uint64_t) gridDim.x * blockDim.x)
 		ent[i * stride] &= ~GG_HT_MATCHED;
-}
-
-int gg_probe_kernel_prepare(gg_scanagg *p)
-{
-	if (p->mode == MODE_HASH)
-		GG_CUDA(cudaFuncSetAttribute(gg_joinhash_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) p->smem));
-	else if (p->mode == MODE_PRIV)
-		GG_CUDA(cudaFuncSetAttribute(gg_joinprobe_kernel<MODE_PRIV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) p->smem));
-	else if (p->mode == MODE_TR)
-		GG_CUDA(cudaFuncSetAttribute(gg_joinprobe_kernel<MODE_TR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) p->smem));
-	else
-		GG_CUDA(cudaFuncSetAttribute(gg_joinprobe_kernel<MODE_TRN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) p->smem));
-	return GG_OK;
-}
-
-int gg_probe_kernel_launch(gg_scanagg *p, const ScanAggParams &prm, cudaStream_t st)
-{
-	if (p->mode == MODE_HASH) gg_joinhash_kernel<<<p->grid, p->threads, p->smem, st>>>(p->prog, prm);
-	else if (p->mode == MODE_PRIV) gg_joinprobe_kernel<MODE_PRIV><<<p->grid, p->threads, p->smem, st>>>(p->prog, prm);
-	else if (p->mode == MODE_TR) gg_joinprobe_kernel<MODE_TR><<<p->grid, p->threads, p->smem, st>>>(p->prog, prm);
-	else gg_joinprobe_kernel<MODE_TRN><<<p->grid, p->threads, p->smem, st>>>(p->prog, prm);
-	GG_CUDA(cudaGetLastError());
-	return GG_OK;
 }
 
 extern "C" {
@@ -167,7 +136,6 @@ int gg_joinagg_create(gg_engine *e, const gg_scan *outer, const gg_scan *inner, 
 	GG_CUDA(cudaMalloc((void **) &j->d_buildcnt, 2 * sizeof(unsigned long long)));
 	GG_CUDA(cudaEventCreate(&j->ev0));
 	GG_CUDA(cudaEventCreate(&j->ev1));
-	GG_CUDA(cudaFuncSetAttribute(gg_joinbuild_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
 	*out = j;
 	return GG_OK;
 }
@@ -231,30 +199,18 @@ int gg_joinagg_build(gg_joinagg *j, gg_relation *inner, uint64_t first_block, ui
 	prm.errflags = j->probe->d_err;
 	prm.snap = e->d_snapshot;
 	prm.counters = j->d_buildcnt;           /* the probe's counters describe the outer side only */
-	const gg_npconfig nc = gg_np_config(7, 2);
-	prm.nstage = nc.nstage;
-	prm.team = nc.team;
-	prm.gcap = 0;
-	const int ncons = nc.ncons;
-	prm.scratch_per_warp = ((j->jp.build.outer.ncols * 64 + 15) & ~15) + 16;
-	prm.scratch_off = (uint32_t) (((size_t) prm.nstage * GG_BLCKSZ + (size_t) prm.nstage * 16 + sizeof(BlockTable) + 15) & ~(size_t) 15);
+	const gg_launch c = gg_np_launch(2, ((j->jp.build.outer.ncols * 64 + 15) & ~15) + 16);
+	prm.nstage = c.nstage;
+	prm.team = c.team;
+	prm.scratch_per_warp = c.scratch_per_warp;
+	prm.scratch_off = c.scratch_off;
 	prm.jt = jt;
 	prm.nrows = inner->nrows;
-	const size_t smem = prm.scratch_off + (size_t) ncons * prm.scratch_per_warp;
-	{
-		char jmsg[512];
-		const int threads = (ncons + 1) * 32;
-		gg_jit_kernel *jk = gg_jit_scanagg(&j->jp.build, MODE_BUILD, threads, e->device, jmsg, sizeof jmsg, -1, 0, nc.forced ? nc.ctas : 0, e->d_snapshot != nullptr);
-		if (jk)
-		{
-			void *args[] = { (void *) &j->jp.build, (void *) &prm };
-			GG_CUDA(cudaFuncSetAttribute((const void *) jk->kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem));
-			GG_CUDA(cudaLaunchKernel((const void *) jk->kernel, dim3(e->sm_count * nc.ctas), dim3(threads), args, smem, st));
-		}
-		else if (threads != 256) { gg_set_error("GGB200_NP_CONFIG needs the run-time specialised kernel: %s", jmsg); return GG_ERR_UNSUPPORTED; }
-		else
-			gg_joinbuild_kernel<<<e->sm_count * 2, 256, smem, st>>>(j->jp.build, prm);
-	}
+	const void *fn = nullptr;
+	int rc = gg_scan_kernel(&j->jp.build, MODE_BUILD, -1, c, e->device, e->d_snapshot != nullptr, &fn);
+	if (rc) return rc;
+	void *args[] = { (void *) &j->jp.build, (void *) &prm };
+	GG_CUDA(cudaLaunchKernel(fn, dim3(e->sm_count * c.ctas), dim3(c.threads), args, c.smem, st));
 	GG_CUDA(cudaGetLastError());
 	e->launches++;
 	GG_CUDA(cudaEventRecord(j->ev1, st));

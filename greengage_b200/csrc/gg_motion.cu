@@ -62,13 +62,11 @@ int gg_partition_rows(gg_engine *e, const gg_scan *scan, const gg_exprpool *pool
 	prm.snap = e->d_snapshot;
 	prm.errflags = (uint32_t *) (d_state + nsegs);
 	prm.counters = d_state + nsegs + 1;
-	const gg_npconfig nc = gg_np_config(7, 2);
-	prm.nstage = nc.nstage;
-	prm.team = nc.team;
-	const int ncons = nc.ncons;
-	const int threads = (ncons + 1) * 32;
-	prm.scratch_per_warp = ((prog.outer.ncols * 64 + 15) & ~15) + 512 + 16;     /* column offsets + the warp's claim windows */
-	prm.scratch_off = (uint32_t) (((size_t) prm.nstage * GG_BLCKSZ + (size_t) prm.nstage * 16 + sizeof(BlockTable) + 15) & ~(size_t) 15);
+	const gg_launch c = gg_np_launch(2, ((prog.outer.ncols * 64 + 15) & ~15) + 512 + 16);     /* column offsets + the warp's claim windows */
+	prm.nstage = c.nstage;
+	prm.team = c.team;
+	prm.scratch_per_warp = c.scratch_per_warp;
+	prm.scratch_off = c.scratch_off;
 	prm.mo.rows = (unsigned long long *) device_out_rows;
 	prm.mo.cursor = d_state;
 	prm.mo.cap = (out_cap_rows / (uint64_t) nsegs) & ~1ull;      /* even: every region starts 16-byte aligned */
@@ -80,7 +78,7 @@ int gg_partition_rows(gg_engine *e, const gg_scan *scan, const gg_exprpool *pool
 	for (int k = 0; k < nkeys; k++) prm.mo.hashtypes |= (uint32_t) hashtype[k] << (4 * k);
 	{
 		/* claim windows (MotionOut.window): as large as keeps the unused tails of all warps below 1/8 of a region */
-		const uint64_t warps = (uint64_t) e->sm_count * nc.ctas * ncons;
+		const uint64_t warps = (uint64_t) e->sm_count * c.ctas * (c.threads / 32 - 1);
 		const uint64_t w = prm.mo.cap / (warps * 8);
 		uint32_t window = 0;
 		if (nsegs <= 32 && w >= 32) { window = 32; while (window * 2 <= w && window < 1024) window *= 2; }
@@ -88,25 +86,14 @@ int gg_partition_rows(gg_engine *e, const gg_scan *scan, const gg_exprpool *pool
 		if (env && nsegs <= 32) { int v = atoi(env); if (v == 0 || (v >= 32 && v <= 4096)) window = (uint32_t) v; }
 		prm.mo.window = window;
 	}
-	const size_t smem = prm.scratch_off + (size_t) ncons * prm.scratch_per_warp;
-	if (ce == cudaSuccess) ce = cudaFuncSetAttribute(gg_motion_part_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem);
 	if (ce == cudaSuccess) ce = cudaEventRecord(e->ev_start, st);
 	if (ce == cudaSuccess)
 	{
-		char jmsg[512];
-		gg_jit_kernel *jk = gg_jit_scanagg(&prog, MODE_PART, threads, e->device, jmsg, sizeof jmsg, -1, 0, nc.forced ? nc.ctas : 0, e->d_snapshot != nullptr);
-		if (jk)
-		{
-			void *args[] = { (void *) &prog, (void *) &prm };
-			ce = cudaFuncSetAttribute((const void *) jk->kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem);
-			if (ce == cudaSuccess) ce = cudaLaunchKernel((const void *) jk->kernel, dim3(e->sm_count * nc.ctas), dim3(threads), args, smem, st);
-		}
-		else if (threads != 256) { gg_set_error("GGB200_NP_CONFIG needs the run-time specialised kernel: %s", jmsg); return GG_ERR_UNSUPPORTED; }
-		else
-		{
-			gg_motion_part_kernel<<<e->sm_count * 2, 256, smem, st>>>(prog, prm);
-			ce = cudaGetLastError();
-		}
+		const void *fn = nullptr;
+		int rc2 = gg_scan_kernel(&prog, MODE_PART, -1, c, e->device, e->d_snapshot != nullptr, &fn);
+		if (rc2) return rc2;
+		void *args[] = { (void *) &prog, (void *) &prm };
+		ce = cudaLaunchKernel(fn, dim3(e->sm_count * c.ctas), dim3(c.threads), args, c.smem, st);
 		e->launches++;
 	}
 	if (ce == cudaSuccess) ce = cudaEventRecord(e->ev_stop, st);

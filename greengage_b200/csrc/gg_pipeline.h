@@ -12,23 +12,7 @@
 #include "gg_scanagg_kernel.cuh"
 #include "gg_engine.h"
 #include "gg_jit.h"
-
-/* Launch configuration of the kernels that run two small blocks per SM by default (hash build, Motion send, general
- * HashAggregate, the transposed / nullable scan and probe variants): consumer warps per block, ring stages, team size
- * (ScanAggParams.team) and blocks per SM.  GGB200_NP_CONFIG="ncons,stages,team,ctas" overrides it for experiments; block
- * sizes other than the default need the run-time specialised kernel (the interpreter kernels are built for 256 threads). */
-struct gg_npconfig { int ncons, nstage, team, ctas; bool forced; };
-static inline gg_npconfig gg_np_config(int ncons, int nstage)
-{
-	gg_npconfig c = { ncons, nstage, 0, 2, false };
-	const char *env = getenv("GGB200_NP_CONFIG");
-	int a, b, t = 0, k = 2;
-	if (env && sscanf(env, "%d,%d,%d,%d", &a, &b, &t, &k) >= 2 && a >= 1 && a <= 30 && b >= 2 && b <= 6 && t >= 0 && t <= a && k >= 1 && k <= 4)
-	{ c.ncons = a; c.nstage = b; c.team = t; c.ctas = k; c.forced = true; }
-	/* at most one team per ring slot (a team's pages arrive on its own barrier set, BlockTable::teamfull) */
-	if (c.team > 0 && c.ncons / c.team > c.nstage) c.ncons = c.team * c.nstage;
-	return c;
-}
+#include "gg_launch.h"
 
 #define GG_MERGE_CAP 1024          /* merged groups the fast path holds per segment */
 #define GG_STREAM_CHUNK_BLOCKS 8192 /* 256 MB staging chunks for gg_scanagg_run_host */
@@ -40,21 +24,18 @@ struct gg_scanagg {
 	gg_exprpool pool;
 	ggp_program prog;
 	ggp_aggmap aggmap[GG_MAX_AGGS];
-	int grid = 0, threads = 0, nstage = 0, scratch_per_warp = 0;
 	int mode = ggd::MODE_PRIV;           /* kernel variant; escalates PRIV -> TR when a run overflows its group capacity */
-	int ctas_per_sm = 2, gcap = 0;
-	uint32_t scratch_off = 0, cnt_off = 0, acc_off = 0;
+	gg_launch cfg;                       /* launch shape of the current variant */
+	int grid = 0;
 	std::vector<std::pair<cudaEvent_t, cudaEvent_t>> kev;   /* events around every scan kernel launch since reset */
 	size_t kev_used = 0;
+	const void *kernel = nullptr;   /* the kernel of the current variant: jit's, or the interpreter instance of the role */
 	gg_jit_kernel *jit = nullptr;   /* plan-specialised kernel for the current variant, or nullptr: interpreter */
-	gg_jit_kernel *jit_snap = nullptr;  /* the same with the snapshot rule built in (gg_jit.h mvcc), compiled when a launch first finds
-	                                     * the engine holding a snapshot; follows `jit` through every reconfiguration */
-	const gg_jit_kernel *jit_snap_of = nullptr;     /* the `jit` that jit_snap was compiled next to */
-	int regslots = -1;              /* private-accumulator variant: trailing value slots kept in registers (-1: not decided) */
+	gg_jit_kernel *jit_snap = nullptr;  /* the same with the snapshot rule built in (gg_jit.h mvcc), or `jit` when there is none;
+	                                     * chosen when a launch first finds the engine holding a snapshot, reset by every
+	                                     * reconfiguration */
 	int chunks_per_page = 0;        /* 32-row chunks per page of the relation being scanned (0: not sampled yet) */
 	int items_per_page = 0;         /* line pointers of the sampled page */
-	int team = 0;                   /* consumer warps per team (ScanAggParams.team); 0: chunks dealt across all warps */
-	bool np_forced = false;         /* launch configuration came from GGB200_NP_CONFIG */
 	bool is_join = false;           /* probe side of a gg_joinagg: prog = the probe program, jt = the built table */
 	ggd::HashAggTable ha = {};           /* MODE_HASH: the group table in HBM */
 	void *ha_mem = nullptr;
@@ -62,7 +43,6 @@ struct gg_scanagg {
 	unsigned long long *d_nout64 = nullptr;
 	ggd::JoinTable jt = {};
 	int join_probe_pc = -1;
-	size_t smem = 0;
 	/* device state */
 	ggp_grec *recs = nullptr;       /* [GG_MERGE_CAP (previous merged)] ++ [grid * GGP_FAST_GROUPS (block records)] */
 	ggp_grec *merged = nullptr;     /* [GG_MERGE_CAP] output of the merge kernel */
@@ -102,6 +82,13 @@ int gg_partition_rows(gg_engine *e, const gg_scan *scan, const gg_exprpool *pool
                       int nsegs, int route, int shift, gg_relation *r, uint64_t first_block, uint64_t nblocks,
                       void *device_out_rows, uint64_t out_cap_rows,
                       uint64_t *host_counts, uint64_t *host_offsets);
-/* gg_join.cu: the probe-side kernels of a join pipeline (interpreter path) */
-int gg_probe_kernel_prepare(gg_scanagg *p);
-int gg_probe_kernel_launch(gg_scanagg *p, const ggd::ScanAggParams &prm, cudaStream_t st);
+/* The kernel that runs the scan kernel body in role `mode` (probe_pc >= 0: the probe side of a join) with launch shape `c`: the
+ * plan-specialised kernel (gg_jit_scanagg: build-time plan cache or NVRTC; mvcc: with the snapshot rule) when there is one, else
+ * the interpreter instance of the role, made ready for c.smem bytes of dynamic shared memory.  Launch it with
+ * cudaLaunchKernel(*fn, grid, c.threads, { &prog, &params }, c.smem).  *jit (optional): the specialised kernel, or nullptr. */
+int gg_scan_kernel(const ggp_program *prog, int mode, int probe_pc, const gg_launch &c, int device, bool mvcc, const void **fn, gg_jit_kernel **jit = nullptr);
+
+/* the interpreter instances of the join and Motion roles (gg_join.cu, gg_motion.cu), for gg_scan_kernel's table */
+__global__ void gg_joinhash_kernel(const __grid_constant__ ggp_program P, const ggd::ScanAggParams prm);
+__global__ void gg_joinbuild_kernel(const __grid_constant__ ggp_program P, const ggd::ScanAggParams prm);
+__global__ void gg_motion_part_kernel(const __grid_constant__ ggp_program P, const ggd::ScanAggParams prm);

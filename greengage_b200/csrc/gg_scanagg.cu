@@ -20,6 +20,15 @@ gg_scanagg_kernel(const __grid_constant__ ggp_program P, const ScanAggParams prm
 	scanagg_body<MODE, DynPlan>(P, prm);
 }
 
+/* HashJoin probe side: the same scan front end; every outer row probes the join hash table and each
+ * match runs the per-match piece of the program (join qual, grouping keys, aggregate arguments) */
+template <int MODE>
+__global__ void __launch_bounds__(MODE == MODE_PRIV ? 704 : 256, MODE == MODE_PRIV ? 1 : 2)
+gg_joinprobe_kernel(const __grid_constant__ ggp_program P, const ScanAggParams prm)
+{
+	scanagg_body<MODE, DynPlan, true>(P, prm);
+}
+
 /* general HashAggregate (any number of groups): scan + probe side variants */
 __global__ void __launch_bounds__(256, 2)
 gg_hashagg_kernel(const __grid_constant__ ggp_program P, const ScanAggParams prm)
@@ -272,174 +281,55 @@ gg_merge_recs_kernel(const ggp_grec *recs, int nrecs, int nkeys, int nacc, ggp_a
 #include "gg_pipeline.h"
 #include "gg_groups.h"
 
-/* launch configuration and shared-memory layout for the current kernel variant:
- *   ring[nstage][32 KB] | full/empty mbarriers | BlockTable | per-warp scratch | (PRIV) counts | (PRIV) sums */
+static_assert(sizeof(BlockTable) == GG_BLOCKTABLE_BYTES && GG_REG_GROUPS == 4, "gg_launch.h sizes the shared memory with these");
+static_assert((int) GGL_PRIV == MODE_PRIV && (int) GGL_TR == MODE_TR && (int) GGL_TRN == MODE_TRN && (int) GGL_BUILD == MODE_BUILD &&
+              (int) GGL_PART == MODE_PART && (int) GGL_HASH == MODE_HASH, "gg_launch.h names the kernel roles");
+
+/* the interpreter instance of every role: [join][mode] */
+static const void *const interp_kernels[2][6] = {
+	{ (const void *) gg_scanagg_kernel<MODE_PRIV>, (const void *) gg_scanagg_kernel<MODE_TR>, (const void *) gg_scanagg_kernel<MODE_TRN>,
+	  (const void *) gg_joinbuild_kernel, (const void *) gg_motion_part_kernel, (const void *) gg_hashagg_kernel },
+	{ (const void *) gg_joinprobe_kernel<MODE_PRIV>, (const void *) gg_joinprobe_kernel<MODE_TR>, (const void *) gg_joinprobe_kernel<MODE_TRN>,
+	  nullptr, nullptr, (const void *) gg_joinhash_kernel },
+};
+
+/* the plan-specialised kernel for a launch shape, or nullptr (why: jmsg) */
+static gg_jit_kernel *scan_jit(const ggp_program *prog, int mode, int probe_pc, const gg_launch &c, int device, bool mvcc, char *jmsg, int jlen)
+{
+	return gg_jit_scanagg(prog, mode, c.threads, device, jmsg, jlen, probe_pc, c.regslots,
+	                      c.forced || (mode == MODE_PRIV && c.ctas > 1) ? c.ctas : 0, mvcc);
+}
+
+int gg_scan_kernel(const ggp_program *prog, int mode, int probe_pc, const gg_launch &c, int device, bool mvcc, const void **fn, gg_jit_kernel **jit)
+{
+	char jmsg[512];
+	gg_jit_kernel *jk = scan_jit(prog, mode, probe_pc, c, device, mvcc, jmsg, sizeof jmsg);
+	if (jit) *jit = jk;
+	if (!jk && getenv("GGB200_JIT_VERBOSE")) fprintf(stderr, "ggb200: interpreter kernel in use (%s)\n", jmsg);
+	if (!jk && mode != MODE_PRIV && c.threads != 256) { gg_set_error("GGB200_NP_CONFIG needs the run-time specialised kernel: %s", jmsg); return GG_ERR_UNSUPPORTED; }
+	*fn = jk ? (const void *) jk->kernel : interp_kernels[probe_pc >= 0][mode];
+	GG_CUDA(cudaFuncSetAttribute(*fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) c.smem));
+	return GG_OK;
+}
+
+/* launch configuration (gg_launch.h gg_scan_config) and kernel for the current variant */
 static int scanagg_configure(gg_scanagg *p)
 {
 	gg_engine *e = p->eng;
-	const int V = p->prog.nslots > 0 ? p->prog.nslots : 1;
-	/* value slots that need shared memory: the private-accumulator variant keeps the last few in registers when a
-	 * plan-specialised kernel is available and the planner expects no more groups than the registers hold */
-	if (p->mode != MODE_PRIV) p->regslots = 0;
-	else if (p->regslots < 0)
+	const int probe_pc = p->is_join ? p->join_probe_pc : -1;
+	if (!gg_scan_config(p->cfg, p->mode, p->is_join, p->prog, p->chunks_per_page, p->items_per_page,
+	                    gg_priv_regslots(&p->prog, p->mode, p->agg.numGroups, probe_pc), e->smem_optin))
+	{ gg_set_error("plan needs too much shared memory"); return GG_ERR_UNSUPPORTED; }
+	p->grid = e->sm_count * p->cfg.ctas;
+	p->jit_snap = nullptr;
+	int rc = gg_scan_kernel(&p->prog, p->mode, probe_pc, p->cfg, e->device, false, &p->kernel, &p->jit);
+	if (rc) return rc;
+	if (!p->jit && p->cfg.regslots > 0)
 	{
-		/* Measured with scripts/dev_regs.sh (10^8-row lineitem-wide): register slots cost a few predicated adds per row
-		 * but free shared memory — Q1 one-stage: 20 warps instead of 16 on the 4-page ring; Q1 PARTIAL stage (8 value
-		 * slots): 16 warps / 4 pages instead of 13 / 3, both faster.  Dense pages run on a 3-page ring where everything
-		 * fits anyway, and there the plain layout is faster. */
-		const int rule = gg_priv_regslots(&p->prog, p->mode, p->agg.numGroups, p->is_join ? p->join_probe_pc : -1);
-		p->regslots = rule;
-		if (p->chunks_per_page >= 10)
-		{
-			/* dense pages: plain layout whenever it leaves room for (nearly) all 20 warps on the 3-page ring */
-			const size_t per_warp = (size_t) ((p->prog.outer.ncols * 64 + 15) & ~15) + (size_t) 32 * (8 * p->prog.nslots + 4) * 4;
-			const size_t ring = (size_t) 3 * GG_BLCKSZ + 3 * 16 + sizeof(BlockTable) + 48;
-			if (ring + 18 * per_warp <= e->smem_optin) p->regslots = 0;
-		}
+		/* the interpreter kernel addresses value slots dynamically: everything in shared memory */
+		p->cfg.regslots = 0;
+		return scanagg_configure(p);
 	}
-	const int nslots = p->prog.nslots - p->regslots;
-	int scr = (p->prog.outer.ncols * 64 + 15) & ~15;             /* column offsets [ncols][32] u16 */
-	if (p->mode == MODE_TR || p->mode == MODE_TRN) scr += V * 33 * 8 + 128 + 128;      /* + transposed values, group ids, null masks */
-	scr = (scr + 15) & ~15;
-	/* datum-row plans can be fed from column files (gg_scanagg_run_aocs): 32 staged rows per warp at the tail of its scratch */
-	if (p->prog.outer.rowwords) scr += 32 * ((p->prog.outer.rowwords | 1) * 8);
-	p->scratch_per_warp = (scr + 15) & ~15;
-	p->nstage = 3;
-	if (p->mode == MODE_PRIV)
-	{
-		/* 1 CTA/SM: 14 consumer warps + producer.  What the ring and the scratch leave of the 227 KB goes to
-		 * the per-thread private accumulators; that fixes how many groups this variant holds. */
-		p->ctas_per_sm = 1;
-		/* Measured on 10^8-row lineitem (scripts/dev_sweep.sh): sparse pages (190 rows = 6 chunks of 32 line pointers)
-		 * need pages in flight more than warps -> 16 consumer warps on a 4-page ring (faster than 20 warps / 3 pages);
-		 * dense pages (430 rows = 14 chunks) keep every warp busy from fewer pages -> 20 warps on a 3-page ring
-		 * (faster than 16 warps / 4 pages).  Fewer warps if the private accumulators of >= 4 groups need the room. */
-		auto fit = [&](int stages, int want) {           /* most consumer warps (<= want) whose accumulators of 4 groups fit */
-			int w = want;
-			for (; w > 4; w--)
-			{
-				size_t need = (size_t) stages * GG_BLCKSZ + (size_t) stages * 16 + sizeof(BlockTable) + 48 +
-				              (size_t) w * p->scratch_per_warp + (size_t) w * 32 * (8 * nslots + 4) * 4;
-				if (need <= e->smem_optin) break;
-			}
-			return w;
-		};
-		int ncons;
-		if (p->chunks_per_page >= 10) { p->nstage = 3; ncons = fit(3, 20); }
-		else
-		{
-			/* plans with many value slots (a PARTIAL-stage Q1 carries 8): when 4 stages leave room for fewer than 15
-			 * warps, a 3-page ring with more warps measured faster (13 warps / 3 pages against 9 / 4) */
-			p->nstage = 4; ncons = fit(4, p->regslots > 0 ? 20 : 16);
-			/* a fifth page in flight when it costs no warp (measured faster for one-stage Q1 with register slots) */
-			if (fit(5, ncons) >= ncons) p->nstage = 5;
-			if (ncons < 15) { int w3 = fit(3, 16); if (w3 >= ncons + 3) { p->nstage = 3; ncons = w3; } }
-		}
-		{
-			const char *cfg = getenv("GGB200_PRIV_CONFIG");     /* "conswarps,stages[,team[,ctas]]" for experiments */
-			int a, b, c = 0, d = 1;
-			p->team = 0;
-			/* Teams (gg_scanagg_kernel.cuh): sparse pages — every chunk of a page gets its own warp, the teams work on different
-			 * pages of the ring.  The team must cover the fullest page (a warp with two chunks holds its whole team back): the
-			 * sampled page's line pointers + 8 %.  Measured on 10^8-row lineitem-wide (190 +- 6 rows per page, scripts/
-			 * sweep_teams.py): 3 teams of 7 on a 5-page ring beat 20 warps dealt across pages, and teams of 6 (pages with 193+
-			 * rows cost a warp two chunks) were slower than both. */
-			if (p->chunks_per_page >= 2 && p->chunks_per_page <= 10 && p->items_per_page > 0 && !p->prog.outer.rowwords && !p->is_join)
-			{
-				const int ts = (p->items_per_page + p->items_per_page / 12 + 31) / 32;
-				int nteams = ts > 0 ? 21 / ts : 0;
-				if (nteams > 5) nteams = 5;
-				if (nteams >= 1 && ts <= 10)
-				{
-					const int want = ts * nteams;
-					int st = 5;
-					while (st > nteams && fit(st, want) < want) st--;
-					if (st >= nteams && fit(st, want) >= want) { ncons = want; p->nstage = st; p->team = ts; }
-				}
-			}
-			if (cfg && sscanf(cfg, "%d,%d,%d,%d", &a, &b, &c, &d) >= 2 && a >= 1 && a <= 30 && b >= 2 && b <= 6 && c >= 0 && c <= a && d >= 1 && d <= 2)
-			{ ncons = a; p->nstage = b; p->team = c; p->ctas_per_sm = d; }
-			/* a team waits for ITS page's phase of a ring slot; an mbarrier tells the current phase from the previous one only,
-			 * so no two teams may be queued on one slot: at most as many teams as stages */
-			if (p->team > 0 && ncons / p->team > p->nstage) ncons = p->team * p->nstage;
-		}
-		p->threads = (ncons + 1) * 32;
-		const int NT = ncons * 32;
-		size_t fixed = (size_t) p->nstage * GG_BLCKSZ + (size_t) p->nstage * 16 + sizeof(BlockTable) + 16 +
-		               (size_t) ncons * p->scratch_per_warp + 16;
-		/* two blocks per SM (experiments: more warps in flight for the latency-bound probe): each gets half, 1 KB reserved per block */
-		const size_t budget = p->ctas_per_sm > 1 ? (e->smem_optin + 1024) / (size_t) p->ctas_per_sm - 1024 : e->smem_optin;
-		if (fixed + (size_t) NT * (8 * nslots + 4) > budget) { gg_set_error("plan needs too much shared memory"); return GG_ERR_UNSUPPORTED; }
-		int gcap = (int) ((budget - fixed) / ((size_t) NT * (8 * nslots + 4)));
-		if (gcap > GGP_FAST_GROUPS) gcap = GGP_FAST_GROUPS;
-		if (p->regslots > 0 && gcap > GG_REG_GROUPS) gcap = GG_REG_GROUPS;
-		p->gcap = gcap;
-		p->scratch_off = (uint32_t) (((size_t) p->nstage * GG_BLCKSZ + (size_t) p->nstage * 16 + sizeof(BlockTable) + 15) & ~(size_t) 15);
-		p->cnt_off = p->scratch_off + (uint32_t) ncons * p->scratch_per_warp;
-		p->acc_off = (p->cnt_off + (uint32_t) gcap * NT * 4 + 15) & ~15u;
-		p->smem = p->acc_off + (size_t) gcap * nslots * NT * 8;
-	}
-	else
-	{
-		/* 2 CTAs/SM x (7 consumer warps + producer = 8 warps) unless configured otherwise */
-		const gg_npconfig nc = gg_np_config(7, 3);
-		p->ctas_per_sm = nc.ctas;
-		p->threads = (nc.ncons + 1) * 32;
-		p->nstage = nc.nstage;
-		p->team = nc.team;
-		p->np_forced = nc.forced;
-		const int ncons = nc.ncons;
-		p->gcap = GGP_MAX_PAIRS / V < GGP_FAST_GROUPS ? GGP_MAX_PAIRS / V : GGP_FAST_GROUPS;
-		p->scratch_off = (uint32_t) (((size_t) p->nstage * GG_BLCKSZ + (size_t) p->nstage * 16 + sizeof(BlockTable) + 15) & ~(size_t) 15);
-		p->cnt_off = p->acc_off = 0;
-		const size_t per_cta = (e->smem_optin + 1024) / (size_t) nc.ctas - 1024;   /* 1 KB reserved per CTA */
-		p->smem = p->scratch_off + (size_t) ncons * p->scratch_per_warp;
-		if (p->smem > per_cta && !nc.forced)
-		{
-			p->nstage = 2;
-			p->scratch_off = (uint32_t) (((size_t) p->nstage * GG_BLCKSZ + (size_t) p->nstage * 16 + sizeof(BlockTable) + 15) & ~(size_t) 15);
-			p->smem = p->scratch_off + (size_t) ncons * p->scratch_per_warp;
-		}
-		if (p->smem > per_cta) { gg_set_error("plan needs too much shared memory"); return GG_ERR_UNSUPPORTED; }
-		if (p->smem < 32 * 1024) p->smem = 32 * 1024;             /* the epilogue reuses the ring as reduction scratch */
-		if ((size_t) ncons * GGP_MAX_PAIRS * 24 > p->smem) p->smem = (size_t) ncons * GGP_MAX_PAIRS * 24;    /* Red[ncons][GGP_MAX_PAIRS] */
-	}
-	p->grid = e->sm_count * p->ctas_per_sm;
-	if (p->mode == MODE_HASH || p->is_join)
-	{
-		char jmsg[512];
-		p->jit = gg_jit_scanagg(&p->prog, p->mode, p->threads, e->device, jmsg, sizeof jmsg, p->is_join ? p->join_probe_pc : -1, 0,
-		                        (p->mode != MODE_PRIV && p->np_forced) || (p->mode == MODE_PRIV && p->ctas_per_sm > 1) ? p->ctas_per_sm : 0);
-		if (!p->jit && getenv("GGB200_JIT_VERBOSE")) fprintf(stderr, "ggb200: interpreter kernel in use (%s)\n", jmsg);
-		if (!p->jit && p->mode != MODE_PRIV && p->threads != 256) { gg_set_error("GGB200_NP_CONFIG needs the run-time specialised kernel: %s", jmsg); return GG_ERR_UNSUPPORTED; }
-		if (p->jit) GG_CUDA(cudaFuncSetAttribute((const void *) p->jit->kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) p->smem));
-	}
-	if (p->is_join) return gg_probe_kernel_prepare(p);
-	if (p->mode == MODE_HASH)
-	{
-		GG_CUDA(cudaFuncSetAttribute(gg_hashagg_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) p->smem));
-		return GG_OK;
-	}
-	{
-		char jmsg[512];
-		p->jit = gg_jit_scanagg(&p->prog, p->mode, p->threads, e->device, jmsg, sizeof jmsg, -1, p->regslots,
-		                        (p->mode != MODE_PRIV && p->np_forced) || (p->mode == MODE_PRIV && p->ctas_per_sm > 1) ? p->ctas_per_sm : 0);
-		if (!p->jit && getenv("GGB200_JIT_VERBOSE")) fprintf(stderr, "ggb200: interpreter kernel in use (%s)\n", jmsg);
-		if (!p->jit && p->mode != MODE_PRIV && p->threads != 256) { gg_set_error("GGB200_NP_CONFIG needs the run-time specialised kernel: %s", jmsg); return GG_ERR_UNSUPPORTED; }
-		if (!p->jit && p->regslots > 0)
-		{
-			/* the interpreter kernel addresses value slots dynamically: everything in shared memory */
-			p->regslots = 0;
-			return scanagg_configure(p);
-		}
-		if (p->jit) GG_CUDA(cudaFuncSetAttribute((const void *) p->jit->kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) p->smem));
-	}
-	if (p->mode == MODE_PRIV)
-		GG_CUDA(cudaFuncSetAttribute(gg_scanagg_kernel<MODE_PRIV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) p->smem));
-	else if (p->mode == MODE_TR)
-		GG_CUDA(cudaFuncSetAttribute(gg_scanagg_kernel<MODE_TR>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) p->smem));
-	else
-		GG_CUDA(cudaFuncSetAttribute(gg_scanagg_kernel<MODE_TRN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) p->smem));
 	return GG_OK;
 }
 
@@ -488,17 +378,17 @@ int scanagg_launch(gg_scanagg *p, const uint8_t *dev_pages, uint64_t nblocks, cu
 	prm.block_recs = p->recs + GG_MERGE_CAP;
 	prm.errflags = p->d_err;
 	prm.counters = p->d_counters;
-	prm.nstage = p->nstage;
-	prm.gcap = p->gcap;
-	prm.scratch_per_warp = p->scratch_per_warp;
-	prm.scratch_off = p->scratch_off;
-	prm.cnt_off = p->cnt_off;
-	prm.acc_off = p->acc_off;
+	prm.nstage = p->cfg.nstage;
+	prm.gcap = p->cfg.gcap;
+	prm.scratch_per_warp = p->cfg.scratch_per_warp;
+	prm.scratch_off = p->cfg.scratch_off;
+	prm.cnt_off = p->cfg.cnt_off;
+	prm.acc_off = p->cfg.acc_off;
 	prm.jt = p->jt;
 	memset(&prm.mo, 0, sizeof prm.mo);
 	prm.nrows = nrows;
 	prm.fill_inner = fill_inner ? 1 : 0;
-	prm.team = p->team;
+	prm.team = p->cfg.team;
 	prm.snap = e->d_snapshot;
 	{
 		const char *kc = getenv("GGB200_KEYCACHE");
@@ -523,54 +413,32 @@ int scanagg_launch(gg_scanagg *p, const uint8_t *dev_pages, uint64_t nblocks, cu
 	}
 	GG_CUDA(cudaEventRecord(p->kev[p->kev_used].first, st));
 	if (p->is_join && !p->jt.ent) { gg_set_error("probe before build"); return GG_ERR_ARG; }
-	if (p->jit)
+	const void *fn = p->kernel;
+	if (p->jit && e->d_snapshot)
 	{
-		/* plan-specialised kernel (any role).  With a snapshot on the engine the scan needs the kernel that carries the snapshot
-		 * rule; the plain one raises GGP_EF_VISIBILITY for every tuple whose hint bits do not decide. */
-		gg_jit_kernel *jk = p->jit;
-		if (e->d_snapshot)
+		/* With a snapshot on the engine the scan needs the specialised kernel that carries the snapshot rule; the plain one raises
+		 * GGP_EF_VISIBILITY for every tuple whose hint bits do not decide (the interpreter kernels carry the rule) */
+		if (!p->jit_snap)
 		{
-			if (p->jit_snap_of != p->jit)
+			char jmsg[512];
+			p->jit_snap = scan_jit(&p->prog, p->mode, p->is_join ? p->join_probe_pc : -1, p->cfg, e->device, true, jmsg, sizeof jmsg);
+			if (p->jit_snap) GG_CUDA(cudaFuncSetAttribute((const void *) p->jit_snap->kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) p->cfg.smem));
+			else
 			{
-				char jmsg[512];
-				p->jit_snap = gg_jit_scanagg(&p->prog, p->mode, p->threads, e->device, jmsg, sizeof jmsg, p->is_join ? p->join_probe_pc : -1, p->regslots,
-				                             (p->mode != MODE_PRIV && p->np_forced) || (p->mode == MODE_PRIV && p->ctas_per_sm > 1) ? p->ctas_per_sm : 0, 1);
-				p->jit_snap_of = p->jit;
-				if (p->jit_snap) GG_CUDA(cudaFuncSetAttribute((const void *) p->jit_snap->kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) p->smem));
-				else if (getenv("GGB200_JIT_VERBOSE")) fprintf(stderr, "ggb200: no specialised kernel with the snapshot rule (%s)\n", jmsg);
+				if (getenv("GGB200_JIT_VERBOSE")) fprintf(stderr, "ggb200: no specialised kernel with the snapshot rule (%s)\n", jmsg);
+				p->jit_snap = p->jit;        /* undecided tuples make the scan fail, never pass */
 			}
-			if (p->jit_snap) jk = p->jit_snap;       /* else: the plain kernel; undecided tuples make the scan fail, never pass */
 		}
-		void *args[] = { (void *) &p->prog, (void *) &prm };
-		GG_CUDA(cudaLaunchKernel((const void *) jk->kernel, dim3(p->grid), dim3(p->threads), args, p->smem, st));
+		fn = (const void *) p->jit_snap->kernel;
 	}
-	else if (p->is_join)
-	{
-		int rcj = gg_probe_kernel_launch(p, prm, st);            /* gg_join.cu */
-		if (rcj) return rcj;
-	}
-	else if (p->mode == MODE_HASH)
-		gg_hashagg_kernel<<<p->grid, p->threads, p->smem, st>>>(p->prog, prm);
-	else if (p->mode == MODE_PRIV)
-		gg_scanagg_kernel<MODE_PRIV><<<p->grid, p->threads, p->smem, st>>>(p->prog, prm);
-	else if (p->mode == MODE_TR)
-		gg_scanagg_kernel<MODE_TR><<<p->grid, p->threads, p->smem, st>>>(p->prog, prm);
-	else
-		gg_scanagg_kernel<MODE_TRN><<<p->grid, p->threads, p->smem, st>>>(p->prog, prm);
-	if (p->mode == MODE_HASH)
-	{
-		/* the group table lives in HBM across launches: nothing to fold */
-		GG_CUDA(cudaGetLastError());
-		GG_CUDA(cudaEventRecord(p->kev[p->kev_used].second, st));
-		p->kev_used++;
-		e->launches++;
-		p->has_state = true;
-		return GG_OK;
-	}
+	void *args[] = { (void *) &p->prog, (void *) &prm };
+	GG_CUDA(cudaLaunchKernel(fn, dim3(p->grid), dim3(p->cfg.threads), args, p->cfg.smem, st));
 	GG_CUDA(cudaGetLastError());
 	GG_CUDA(cudaEventRecord(p->kev[p->kev_used].second, st));
 	p->kev_used++;
 	e->launches++;
+	p->has_state = true;
+	if (p->mode == MODE_HASH) return GG_OK;         /* the group table lives in HBM across launches: nothing to fold */
 	/* fold the block records (and the previously merged groups) */
 	ggp_acckinds kinds;
 	memcpy(kinds.k, p->prog.acckind, sizeof kinds.k);
@@ -582,7 +450,6 @@ int scanagg_launch(gg_scanagg *p, const uint8_t *dev_pages, uint64_t nblocks, cu
 	 * by copying the whole (zero-initialised) merged array */
 	GG_CUDA(cudaMemcpyAsync(p->recs, p->merged, sizeof(ggp_grec) * GG_MERGE_CAP, cudaMemcpyDeviceToDevice, st));
 	GG_CUDA(cudaMemsetAsync(p->merged, 0, sizeof(ggp_grec) * GG_MERGE_CAP, st));
-	p->has_state = true;
 	return GG_OK;
 }
 
@@ -600,17 +467,15 @@ static int scanagg_adapt_to_pages(gg_scanagg *p, const uint8_t *dev_page, const 
 	int items = pd_lower >= GG_PAGE_HEADER_SIZE && pd_lower <= GG_BLCKSZ ? (int) ((pd_lower - GG_PAGE_HEADER_SIZE) >> 2) : 0;
 	p->chunks_per_page = items > 0 ? (items + 31) / 32 : 1;
 	p->items_per_page = items;
-	p->regslots = -1;                          /* decided again for this page density */
-	const int threads0 = p->threads, stages0 = p->nstage;
+	p->cfg.regslots = -1;                      /* decided again for this page density */
 	int rc = scanagg_configure(p);
 	if (rc) return rc;
-	if (p->mode == MODE_PRIV && p->agg.numGroups > p->gcap)
+	if (p->mode == MODE_PRIV && p->agg.numGroups > p->cfg.gcap)
 	{
 		/* the denser configuration leaves room for fewer groups than the planner expects: keep the default one */
 		p->chunks_per_page = 1;
 		rc = scanagg_configure(p);
 	}
-	(void) threads0; (void) stages0;
 	return rc;
 }
 
@@ -624,22 +489,17 @@ int scanagg_finish_create(gg_scanagg *p, gg_scanagg **out)
 	 * group estimate decides whether they can hold the groups */
 	p->mode = p->prog.nullable ? MODE_TRN : MODE_TR;
 	if (p->prog.priv_ok) p->mode = MODE_PRIV;
-	if (!p->is_join)
-	{
-		const char *force = getenv("GGB200_SCAN_MODE");       /* experiments: 0 PRIV, 1 TR, 2 TRN */
-		if (force) { int m = atoi(force); if (m == MODE_PRIV && !p->prog.priv_ok) m = MODE_TR; if (p->prog.nullable) m = MODE_TRN; p->mode = m; }
-	}
-	{
-		const char *force = getenv("GGB200_SCAN_MODE");
-		if (force && atoi(force) == MODE_HASH) p->mode = MODE_HASH;
-	}
+	const char *force = getenv("GGB200_SCAN_MODE");           /* experiments: 0 PRIV, 1 TR, 2 TRN, 5 HASH */
+	if (force && atoi(force) == MODE_HASH) p->mode = MODE_HASH;
+	else if (force && !p->is_join)
+	{ int m = atoi(force); if (m == MODE_PRIV && !p->prog.priv_ok) m = MODE_TR; if (p->prog.nullable) m = MODE_TRN; p->mode = m; }
 	rc = scanagg_configure(p);
-	if (rc == GG_OK && p->mode == MODE_PRIV && agg->numGroups > p->gcap)
+	if (rc == GG_OK && p->mode == MODE_PRIV && agg->numGroups > p->cfg.gcap)
 	{
 		p->mode = p->prog.nullable ? MODE_TRN : MODE_TR;
 		rc = scanagg_configure(p);
 	}
-	if (rc == GG_OK && p->mode != MODE_HASH && agg->numGroups > p->gcap)
+	if (rc == GG_OK && p->mode != MODE_HASH && agg->numGroups > p->cfg.gcap)
 	{
 		/* the planner expects more groups than a block holds on chip: the HBM hash table from the start */
 		p->mode = MODE_HASH;
@@ -994,6 +854,46 @@ static void finalize_rows(const gg_agg *agg, const ggp_aggmap *aggmap, const ggp
 	}
 }
 
+/* merged group records -> rows (finalize_aggregate, nodeAgg.c:871-999).  Plain aggregation over zero rows still yields one row
+ * (nodeAgg.c:1247-1400), unless `empty_is_empty` (a segment that does not own the result). */
+static int records_to_rows(const gg_agg *agg, const ggp_aggmap *aggmap, const ggp_program *prog, int final_stage, std::vector<ggp_grec> &recs,
+                           long long n, bool empty_is_empty, gg_aggrow *out, int outcap, int *nout)
+{
+	if (n == 0 && agg->numCols == 0 && !empty_is_empty) { recs.resize(1); memset(&recs[0], 0, sizeof(ggp_grec)); n = 1; }
+	if (n > outcap) { gg_set_error("output capacity %d < %lld groups", outcap, n); return GG_ERR_NOMEM; }
+	finalize_rows(agg, aggmap, prog, final_stage, recs.data(), (int) n, out);
+	*nout = (int) n;
+	return GG_OK;
+}
+
+/* Run the fed inputs again on kernel variant `mode` (MODE_HASH: into a group table of `ha_cap` slots): reconfigure, reset, and
+ * feed everything again — through the batched join's replay_hook when there is one — like the reference's hybrid hash
+ * aggregate re-reading spilled input (execHHashagg.c:1093). */
+static int scanagg_replay(gg_scanagg *p, int mode, uint64_t ha_cap)
+{
+	gg_engine *e = p->eng;
+	std::vector<gg_scanagg::Fed> replay = p->fed;
+	p->mode = mode;
+	int rc = scanagg_configure(p);
+	if (rc) return rc;
+	p->nrecs_total = GG_MERGE_CAP + p->grid * GGP_FAST_GROUPS;
+	if (mode == MODE_HASH)
+	{
+		p->ha_cap = ha_cap;
+		if (p->ha_mem) { GG_CUDA(cudaStreamSynchronize(e->stream)); cudaFree(p->ha_mem); p->ha_mem = nullptr; }
+	}
+	rc = gg_scanagg_reset(p);
+	if (rc) return rc;
+	if (p->replay_hook) return p->replay_hook();
+	for (const auto &f : replay)
+	{
+		rc = f.dev ? scanagg_launch(p, f.dev, f.nblocks, e->stream, f.nrows, f.fill, f.tile_rows) : scanagg_stream_host(p, f.host, f.nblocks);
+		if (rc) return rc;
+	}
+	p->fed = replay;
+	return GG_OK;
+}
+
 int gg_scanagg_fetch(gg_scanagg *p, gg_aggrow *out, int outcap, int *nout,
                      uint64_t *rows_scanned, uint64_t *rows_passed)
 {
@@ -1008,41 +908,30 @@ int gg_scanagg_fetch(gg_scanagg *p, gg_aggrow *out, int outcap, int *nout,
 	uint32_t flags = p->h_mirror->st.err;
 	unsigned long long counters[2] = { p->h_mirror->st.counters[0], p->h_mirror->st.counters[1] };
 	int n = p->h_mirror->st.nout;
-	if (p->mode == MODE_HASH || ((flags & GGP_EF_GROUP_OVERFLOW) && p->mode != MODE_PRIV))
+	/* Escalation, then the inputs are replayed and fetched again.  Private accumulators: more groups than they hold (the
+	 * planner's numGroups was low or absent), or a non-finite private sum, which only the value-tracking transposed variant can
+	 * attribute to an infinite input or to a float8pl overflow.  A block-table variant with more groups than a block holds:
+	 * the general HashAggregate.  Its table full: one 8 times larger. */
+	int next = -1;
+	uint64_t cap = 0;
+	if (p->mode == MODE_PRIV && (flags & (GGP_EF_GROUP_OVERFLOW | GGP_EF_RECHECK))) next = p->prog.nullable ? MODE_TRN : MODE_TR;
+	else if (p->mode != MODE_HASH && (flags & GGP_EF_GROUP_OVERFLOW)) { next = MODE_HASH; cap = p->ha_cap ? p->ha_cap : 1u << 20; }
+	else if (p->mode == MODE_HASH && (flags & GGP_EF_TABLE_FULL)) { next = MODE_HASH; cap = p->ha_cap * 8; }
+	if (next >= 0)
 	{
-		/* the general HashAggregate.  Reached directly (planner expected many groups), or because a block-table
-		 * variant overflowed, or because this table filled up: then the fed inputs are replayed into a larger one. */
-		const bool grow = p->mode == MODE_HASH && (flags & GGP_EF_TABLE_FULL);
-		if (p->mode != MODE_HASH || grow)
-		{
-			std::vector<gg_scanagg::Fed> replay = p->fed;
-			uint64_t cap = grow ? p->ha_cap * 8 : (p->ha_cap ? p->ha_cap : 1u << 20);
-			if (cap > (1ull << 31)) { gg_set_error("more groups than the device hash aggregate can hold"); return GG_ERR_NOMEM; }
-			p->mode = MODE_HASH;
-			int rc2 = scanagg_configure(p);
-			if (rc2) return rc2;
-			p->ha_cap = cap;
-			if (p->ha_mem) { GG_CUDA(cudaStreamSynchronize(e->stream)); cudaFree(p->ha_mem); p->ha_mem = nullptr; }
-			rc2 = gg_scanagg_reset(p);
-			if (rc2) return rc2;
-			if (p->replay_hook) { rc2 = p->replay_hook(); if (rc2) return rc2; }
-			else
-			{
-				for (const auto &f : replay)
-				{
-					rc2 = f.dev ? scanagg_launch(p, f.dev, f.nblocks, e->stream, f.nrows, f.fill, f.tile_rows) : scanagg_stream_host(p, f.host, f.nblocks);
-					if (rc2) return rc2;
-				}
-				p->fed = replay;
-			}
-			return gg_scanagg_fetch(p, out, outcap, nout, rows_scanned, rows_passed);
-		}
-		if (rows_scanned) *rows_scanned = counters[0];
-		if (rows_passed) *rows_passed = counters[1];
+		if (cap > (1ull << 31)) { gg_set_error("more groups than the device hash aggregate can hold"); return GG_ERR_NOMEM; }
+		int rc = scanagg_replay(p, next, cap);
+		return rc ? rc : gg_scanagg_fetch(p, out, outcap, nout, rows_scanned, rows_passed);
+	}
+	if (rows_scanned) *rows_scanned = counters[0];
+	if (rows_passed) *rows_passed = counters[1];
+	std::vector<ggp_grec> recs;
+	if (p->mode == MODE_HASH)
+	{
+		/* the general HashAggregate: the groups come out of its table */
 		unsigned long long n64 = 0;
 		const unsigned long long ecap = (unsigned long long) (outcap > 0 ? outcap : 1);
 		ggp_grec *d_recs = nullptr;
-		std::vector<ggp_grec> recs;
 		if (p->has_state)
 		{
 			GG_CUDA(cudaMalloc((void **) &d_recs, sizeof(ggp_grec) * ecap));
@@ -1064,53 +953,17 @@ int gg_scanagg_fetch(gg_scanagg *p, gg_aggrow *out, int outcap, int *nout,
 			cudaFree(d_recs);
 			if (ce != cudaSuccess) return gg_cuda_fail(ce, "gg_scanagg_fetch(hash)");
 		}
-		int rc3 = gg_errflags_to_code(flags & ~(uint32_t) GGP_EF_GROUP_OVERFLOW);
-		if (rc3) return rc3;
-		if (n64 > ecap) { gg_set_error("output capacity %d < %llu groups", outcap, n64); return GG_ERR_NOMEM; }
-		if (n64 == 0 && p->agg.numCols == 0) { recs.resize(1); memset(&recs[0], 0, sizeof(ggp_grec)); n64 = 1; }
-		finalize_rows(&p->agg, p->aggmap, &p->prog, 0, recs.data(), (int) n64, out);
-		*nout = (int) n64;
-		return GG_OK;
+		int rc = gg_errflags_to_code(flags & ~(uint32_t) GGP_EF_GROUP_OVERFLOW);
+		if (rc) return rc;
+		return records_to_rows(&p->agg, p->aggmap, &p->prog, 0, recs, (long long) n64, false, out, outcap, nout);
 	}
-	if ((flags & (GGP_EF_GROUP_OVERFLOW | GGP_EF_RECHECK)) && p->mode == MODE_PRIV)
-	{
-		/* Either more groups than the private-accumulator variant holds (the planner's numGroups was low or
-		 * absent), or a non-finite private sum, which only the value-tracking transposed variant can attribute
-		 * to an infinite input or to a float8pl overflow.  Replay the fed inputs on that variant, like the
-		 * reference's hybrid hash aggregate re-reading spilled input (execHHashagg.c:1093). */
-		std::vector<gg_scanagg::Fed> replay = p->fed;
-		p->mode = p->prog.nullable ? MODE_TRN : MODE_TR;
-		int rc2 = scanagg_configure(p);
-		if (rc2) return rc2;
-		p->nrecs_total = GG_MERGE_CAP + p->grid * GGP_FAST_GROUPS;
-		rc2 = gg_scanagg_reset(p);
-		if (rc2) return rc2;
-		if (p->replay_hook) { rc2 = p->replay_hook(); if (rc2) return rc2; }
-		else
-		{
-			for (const auto &f : replay)
-			{
-				rc2 = f.dev ? scanagg_launch(p, f.dev, f.nblocks, e->stream, f.nrows, f.fill, f.tile_rows) : scanagg_stream_host(p, f.host, f.nblocks);
-				if (rc2) return rc2;
-			}
-			p->fed = replay;
-		}
-		return gg_scanagg_fetch(p, out, outcap, nout, rows_scanned, rows_passed);
-	}
-	if (rows_scanned) *rows_scanned = counters[0];
-	if (rows_passed) *rows_passed = counters[1];
 	int rc = gg_errflags_to_code(flags);
 	if (rc) return rc;
 	if (!p->has_state) n = 0;
-	/* plain aggregation over zero rows still yields one row (nodeAgg.c:1247-1400) */
-	std::vector<ggp_grec> recs((size_t) (n > 0 ? n : 1));
+	recs.resize((size_t) (n > 0 ? n : 0));
 	if (n > 0 && n <= GGP_FAST_GROUPS) memcpy(recs.data(), p->h_mirror->recs, sizeof(ggp_grec) * (size_t) n);     /* already here */
 	else if (n > 0) GG_CUDA(cudaMemcpy(recs.data(), p->recs, sizeof(ggp_grec) * n, cudaMemcpyDeviceToHost));
-	if (n == 0 && p->agg.numCols == 0) { memset(&recs[0], 0, sizeof(ggp_grec)); n = 1; }
-	if (n > outcap) { gg_set_error("output capacity %d < %d groups", outcap, n); return GG_ERR_NOMEM; }
-	finalize_rows(&p->agg, p->aggmap, &p->prog, 0, recs.data(), n, out);
-	*nout = n;
-	return GG_OK;
+	return records_to_rows(&p->agg, p->aggmap, &p->prog, 0, recs, n, false, out, outcap, nout);
 }
 
 int gg_scanagg_scan_kernel_ms(gg_scanagg *p, float *ms, int *launches)
@@ -1262,18 +1115,14 @@ int gg_agg_final(gg_engine *e, const gg_agg *agg, const gg_aggrow *in, int nin,
 	if (le == cudaSuccess) le = cudaMemcpyAsync(&n, d_n, sizeof n, cudaMemcpyDeviceToHost, e->stream);
 	if (le == cudaSuccess) le = cudaMemcpyAsync(&flags, d_err, sizeof flags, cudaMemcpyDeviceToHost, e->stream);
 	if (le == cudaSuccess) le = cudaStreamSynchronize(e->stream);
-	std::vector<ggp_grec> merged((size_t) (n > 0 ? n : 1));
+	std::vector<ggp_grec> merged((size_t) (n > 0 ? n : 0));
 	if (le == cudaSuccess && n > 0) le = cudaMemcpy(merged.data(), d_out, sizeof(ggp_grec) * n, cudaMemcpyDeviceToHost);
 	if (le != cudaSuccess) return gg_cuda_fail(le, "gg_agg_final");
 	int rc = gg_errflags_to_code(flags);
 	if (rc) return rc;
-	if (n == 0 && agg->numCols == 0) { memset(&merged[0], 0, sizeof(ggp_grec)); n = 1; }
-	if (n > outcap) { gg_set_error("output capacity %d < %d groups", outcap, n); return GG_ERR_NOMEM; }
 	gg_agg fin = *agg;
 	fin.aggstage = GG_AGGSTAGE_FINAL;
-	finalize_rows(&fin, aggmap, &prog, 1, merged.data(), n, out);
-	*nout = n;
-	return GG_OK;
+	return records_to_rows(&fin, aggmap, &prog, 1, merged, n, false, out, outcap, nout);
 }
 
 
@@ -1414,16 +1263,10 @@ int gg_groups_fetch(gg_groups *g, gg_aggrow *out, int outcap, int *nout, uint64_
 		if (n > 0 && n <= first) memcpy(recs.data(), hr, sizeof(ggp_grec) * (size_t) n);
 		else if (n > 0) GG_CUDA(cudaMemcpy(recs.data(), g->recs, sizeof(ggp_grec) * (size_t) n, cudaMemcpyDeviceToHost));
 	}
-	int n = (int) recs.size();
-	/* plain aggregation over zero rows still yields one row (nodeAgg.c:1247-1400) — on the segment that owns the result */
-	if (n == 0 && g->agg.numCols == 0 && !g->empty_is_empty) { recs.resize(1); memset(&recs[0], 0, sizeof(ggp_grec)); n = 1; }
-	if (n > outcap) { gg_set_error("output capacity %d < %d groups", outcap, n); return GG_ERR_NOMEM; }
 	std::vector<ggp_program> pb(1);
 	memset(&pb[0], 0, sizeof(ggp_program));
 	memcpy(pb[0].keytype, g->keytype, sizeof g->keytype);
-	finalize_rows(&g->agg, g->aggmap, &pb[0], 0, recs.data(), n, out);
-	*nout = n;
-	return GG_OK;
+	return records_to_rows(&g->agg, g->aggmap, &pb[0], 0, recs, (long long) recs.size(), g->empty_is_empty, out, outcap, nout);
 }
 
 int gg_groups_info(gg_groups *g, int *sparse, int *cap)
