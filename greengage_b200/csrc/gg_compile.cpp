@@ -491,7 +491,7 @@ void gen_num(Ctx &c, int root, int want)
 	const gg_expr &e = c.pool->nodes[root];
 	const int own = num_scale(c, root);
 	if (c.failed) return;
-	if (want < own || want > GG_NUM_MAX_SCALE + 3) { fail(c, "numeric expression needs scale %d", want); return; }
+	if (want < own || want > GG_NUM_MAX_SCALE) { fail(c, "numeric expression needs scale %d", want); return; }
 	for (int i = 0; i < c.npersist; i++)
 		if (expr_equal(c.pool, c.persist_root[i], root))
 		{
@@ -503,8 +503,14 @@ void gen_num(Ctx &c, int root, int want)
 	{
 		const int slot = col_slot(c, e.varno, e.varattno);
 		if (c.failed) return;
-		emit(c, GGP_LD_NUM, slot | ((e.varno == 1 && !c.inner_as_outer) ? 0x80 : 0), want & 15);
-		if (want > 15) emit(c, GGP_IMUL_K, add_const(c, kPow10[want - 15], false));
+		if (e.varno == 1 && !c.inner_as_outer)
+		{
+			/* an inner column above a join: the build program stored it at its own scale (ggp_compile_join) */
+			emit(c, GGP_LD_NUM, slot | 0x80, own);
+			if (want > own) emit(c, GGP_IMUL_K, add_const(c, kPow10[want - own], false));
+			return;
+		}
+		emit(c, GGP_LD_NUM, slot, want);
 		return;
 	}
 	if (e.kind == GG_E_CONST) { emit(c, GGP_LD_K, num_const(c, e, want)); return; }
@@ -1097,7 +1103,16 @@ int ggp_compile_join(const gg_scan *outer, const gg_scan *inner, const gg_hashjo
 		int slot = col_slot(b, 1, att + 1);
 		if (b.failed) break;
 		int lt = innerside.coltype[p];
-		emit(b, lt == GGP_LT_I4 ? GGP_LD_C4 : lt == GGP_LT_I8 ? GGP_LD_C8 : lt == GGP_LT_BPCHAR ? GGP_LD_BP : lt == GGP_LT_VARCHAR ? GGP_LD_VS : GGP_LD_BOOL, slot);
+		if (lt == GGP_LT_NUM)
+		{
+			/* a numeric travels as its scaled integer at the column's declared scale; the probe rescales it (gen_num) */
+			const int32_t typmod = inner->desc.attrs[att].atttypmod;
+			const int sc = (typmod - 4) & 0xFFFF;
+			if (typmod < 4 || sc > GG_NUM_MAX_SCALE) { fail(b, "numeric inner column %d: only numeric(p,s) with s <= %d travels above a join", att + 1, GG_NUM_MAX_SCALE); break; }
+			emit(b, GGP_LD_NUM, slot, sc);
+		}
+		else
+			emit(b, lt == GGP_LT_I4 ? GGP_LD_C4 : lt == GGP_LT_I8 ? GGP_LD_C8 : lt == GGP_LT_BPCHAR ? GGP_LD_BP : lt == GGP_LT_VARCHAR ? GGP_LD_VS : GGP_LD_BOOL, slot);
 		ggp_op *o = &jp->build.code[jp->build.ncode - 1];
 		o->flags |= GGP_F_OUT;
 		o->out = (uint8_t) p;

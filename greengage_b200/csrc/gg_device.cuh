@@ -416,15 +416,25 @@ __device__ __forceinline__ int64_t load_numeric(uint32_t p, int scale, uint32_t 
 	if (nd > 8) { err |= GGP_EF_NUMERIC_RANGE; return 0; }                      /* more than 32 decimal digits never fit */
 	uint64_t v = 0;
 	bool bad = false;
-	for (int i = 0; i < nd; i++)
-	{
-		const uint32_t dig = lds8(dp + 2 * i) | (lds8(dp + 2 * i + 1) << 8);
-		if (__umul64hi(v, 10000ull) != 0) bad = true;
-		v = v * 10000ull + dig;
-	}
-	/* v = value * 10000^(nd - 1 - weight); wanted: value * 10^scale */
+	/* value * 10000^(nd - 1 - weight) is v after the loop; wanted: value * 10^scale, so v is then scaled by 10^e.  When the last
+	 * digit reaches 1..3 decimals past the column's scale (a scale that is not a multiple of 4), those decimals are zeros:
+	 * they are dropped from the digit before it is added, so that v never holds more than the scaled value */
 	int e = 4 * (weight - (nd - 1)) + scale;
 	if (nd == 0) e = 0;
+	for (int i = 0; i < nd; i++)
+	{
+		uint32_t dig = lds8(dp + 2 * i) | (lds8(dp + 2 * i + 1) << 8);
+		uint64_t mul = 10000ull;
+		if (i == nd - 1 && e < 0 && e > -4)
+		{
+			const uint32_t drop = e == -1 ? 10u : e == -2 ? 100u : 1000u;
+			if (dig % drop) bad = true;                                         /* digits beyond the column's scale must be zeros */
+			dig /= drop; mul /= drop; e = 0;
+		}
+		const uint64_t m = v * mul;
+		if (__umul64hi(v, mul) != 0 || m + dig < m) bad = true;             /* the product, or the digit's carry, past 2^64 */
+		v = m + dig;
+	}
 	for (; e > 0; e--) { if (__umul64hi(v, 10ull) != 0) bad = true; v *= 10ull; }
 	for (; e < 0; e++) { if (v % 10ull) bad = true; v /= 10ull; }               /* digits beyond the column's scale must be zeros */
 	if (v >> 63) bad = true;
@@ -651,7 +661,8 @@ __device__ __forceinline__ void exec_op(const ggp_op o, const EvalCtx &X, const 
 		{
 			uint32_t e2 = 0;
 			M.accnull = GG_COLNULL(o);
-			M.acc = M.accnull ? 0 : (uint64_t) load_numeric(GG_COLADDR(o), o.aux & 15, e2);
+			/* an inner column above a join: the build program loaded it at its column scale into the payload */
+			M.acc = M.accnull ? 0 : GG_ISINNER(o) ? GG_INNERVAL(o) : (uint64_t) load_numeric(GG_COLADDR(o), o.aux & 15, e2);
 			if (M.live) err |= e2;
 			break;
 		}

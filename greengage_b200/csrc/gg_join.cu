@@ -88,7 +88,8 @@ struct gg_joinagg {
 	bool lasj_empty = false;        /* LASJ_NOTIN met a NULL inner key: the result is empty */
 	float build_ms = 0;
 	cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-	unsigned long long *d_buildcnt = nullptr;   /* rows scanned / passed by the build kernel (kept apart from the probe's counters) */
+	unsigned long long *d_buildcnt = nullptr;   /* rows scanned / passed by the build kernel (kept apart from the probe's counters),
+	                                             * then the build kernel's error flags */
 	/* hybrid hash join (nodeHash.c:713,1132; gg_joinagg_set_work_mem / gg_joinagg_run): the plan as given, and what a
 	 * batched run builds from it */
 	gg_scan outer_scan, inner_scan;
@@ -133,7 +134,7 @@ int gg_joinagg_create(gg_engine *e, const gg_scan *outer, const gg_scan *inner, 
 	if (rc) { delete j; return rc; }
 	j->outer_scan = *outer; j->inner_scan = *inner; j->hj = *hj; j->agg = *agg; j->pool = *pool;
 	GG_CUDA(cudaMalloc((void **) &j->d_cnt, 4 * sizeof(unsigned long long)));      /* line pointers | nbuilt[0..2] (JoinTable) */
-	GG_CUDA(cudaMalloc((void **) &j->d_buildcnt, 2 * sizeof(unsigned long long)));
+	GG_CUDA(cudaMalloc((void **) &j->d_buildcnt, 3 * sizeof(unsigned long long)));      /* rows scanned | passed | error flags */
 	GG_CUDA(cudaEventCreate(&j->ev0));
 	GG_CUDA(cudaEventCreate(&j->ev1));
 	*out = j;
@@ -196,7 +197,9 @@ int gg_joinagg_build(gg_joinagg *j, gg_relation *inner, uint64_t first_block, ui
 	memset(&prm, 0, sizeof prm);
 	prm.pages = pages;
 	prm.nblocks = nblocks;
-	prm.errflags = j->probe->d_err;
+	uint32_t *d_builderr = (uint32_t *) (j->d_buildcnt + 2);
+	GG_CUDA(cudaMemsetAsync(d_builderr, 0, sizeof(uint32_t), st));
+	prm.errflags = d_builderr;
 	prm.snap = e->d_snapshot;
 	prm.counters = j->d_buildcnt;           /* the probe's counters describe the outer side only */
 	const gg_launch c = gg_np_launch(2, ((j->jp.build.outer.ncols * 64 + 15) & ~15) + 16);
@@ -216,7 +219,10 @@ int gg_joinagg_build(gg_joinagg *j, gg_relation *inner, uint64_t first_block, ui
 	GG_CUDA(cudaEventRecord(j->ev1, st));
 	unsigned long long nb[3] = { 0, 0, 0 };
 	GG_CUDA(cudaMemcpyAsync(nb, j->d_cnt + 1, sizeof nb, cudaMemcpyDeviceToHost, st));
+	uint32_t builderr = 0;
+	GG_CUDA(cudaMemcpyAsync(&builderr, d_builderr, sizeof builderr, cudaMemcpyDeviceToHost, st));
 	GG_CUDA(cudaStreamSynchronize(st));
+	j->probe->build_err = builderr & ~(uint32_t) GGP_EF_INFO_MASK;
 	GG_CUDA(cudaEventElapsedTime(&j->build_ms, j->ev0, j->ev1));
 	j->rows_built = nb[0];
 	j->null_keys = nb[1];
@@ -377,13 +383,14 @@ static int joinagg_run_batches(gg_joinagg *j)
 	gg_joinagg *b = j->bj;
 	const int Wo = 1 + j->notargets, Wi = 1 + j->nitargets;
 	j->build_ms = 0; j->rows_built = 0; j->null_keys = 0;
+	uint32_t builderr = 0;          /* every batch's build counts, not only the last one's */
 	for (int k = 0; k < j->nbatch; k++)
 	{
 		gg_relation *irel = nullptr, *orel = nullptr;
 		int rc = gg_relation_attach_rows(j->eng, j->ibuf->pages + (uint64_t) k * j->icap * Wi * 8, j->icounts[(size_t) k], j->nitargets, &irel);
 		if (rc == GG_OK) rc = gg_relation_attach_rows(j->eng, j->obuf->pages + (uint64_t) k * j->ocap * Wo * 8, j->ocounts[(size_t) k], j->notargets, &orel);
 		if (rc == GG_OK) rc = gg_joinagg_build(b, irel, 0, irel->nblocks);
-		if (rc == GG_OK) { j->build_ms += b->build_ms; j->rows_built += b->rows_built; j->null_keys += b->null_keys; }
+		if (rc == GG_OK) { j->build_ms += b->build_ms; j->rows_built += b->rows_built; j->null_keys += b->null_keys; builderr |= b->probe->build_err; b->probe->build_err = builderr; }
 		if (rc == GG_OK && !b->lasj_empty) rc = gg_scanagg_run(b->probe, orel, 0, orel->nblocks);
 		if (rc == GG_OK) rc = joinagg_fill_inner(b);
 		gg_relation_free(irel);
@@ -486,7 +493,13 @@ int gg_joinagg_groups(gg_joinagg *j, gg_groups **out)
 		int rc = joinagg_fill_inner(j);          /* right / full joins: the unmatched inner rows belong to the result */
 		if (rc) return rc;
 	}
-	return gg_scanagg_groups(j->bj && j->nbatch > 1 ? j->bj->probe : j->probe, out);
+	gg_scanagg *p = j->bj && j->nbatch > 1 ? j->bj->probe : j->probe;
+	if (p->build_err)
+	{
+		const int rc = gg_errflags_to_code(p->build_err);         /* the hash table holds a value the device refused */
+		if (rc) return rc;
+	}
+	return gg_scanagg_groups(p, out);
 }
 
 int gg_joinagg_reset(gg_joinagg *j)

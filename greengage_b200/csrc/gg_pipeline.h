@@ -43,6 +43,8 @@ struct gg_scanagg {
 	unsigned long long *d_nout64 = nullptr;
 	ggd::JoinTable jt = {};
 	int join_probe_pc = -1;
+	uint32_t build_err = 0;         /* error flags the join's build kernel raised for the table `jt`: fetch reports them, and
+	                                 * neither a replay nor a reset of the probe side clears them (the table stays as built) */
 	/* device state */
 	ggp_grec *recs = nullptr;       /* [GG_MERGE_CAP (previous merged)] ++ [grid * GGP_FAST_GROUPS (block records)] */
 	ggp_grec *merged = nullptr;     /* [GG_MERGE_CAP] output of the merge kernel */

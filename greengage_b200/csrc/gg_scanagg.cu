@@ -769,8 +769,8 @@ extern "C" int gg_debug_numeric_final(int which, int64_t lo, int64_t hi, int sca
 	return 0;
 }
 
-static void finalize_rows(const gg_agg *agg, const ggp_aggmap *aggmap, const ggp_program *prog, int final_stage,
-                          const ggp_grec *recs, int n, gg_aggrow *out)
+static int finalize_rows(const gg_agg *agg, const ggp_aggmap *aggmap, const ggp_program *prog, int final_stage,
+                         const ggp_grec *recs, int n, gg_aggrow *out)
 {
 	for (int g = 0; g < n; g++)
 	{
@@ -829,8 +829,12 @@ static void finalize_rows(const gg_agg *agg, const ggp_aggmap *aggmap, const ggp
 					{
 						gg_i128 a = 0;
 						int rs = 0;
-						if (!numeric_avg128(sum, aggmap[i].scale, nn, &a, &rs)) { v.isnull = 1; v.pad = 1; }     /* does not fit: flagged, see fetch */
-						else numeric_store(v, a, rs);
+						if (!numeric_avg128(sum, aggmap[i].scale, nn, &a, &rs))
+						{
+							gg_set_error("numeric avg whose quotient does not fit 128 bits at its scale");
+							return GG_ERR_UNSUPPORTED;
+						}
+						numeric_store(v, a, rs);
 					}
 					break;
 				}
@@ -852,6 +856,7 @@ static void finalize_rows(const gg_agg *agg, const ggp_aggmap *aggmap, const ggp
 			}
 		}
 	}
+	return GG_OK;
 }
 
 /* merged group records -> rows (finalize_aggregate, nodeAgg.c:871-999).  Plain aggregation over zero rows still yields one row
@@ -861,7 +866,8 @@ static int records_to_rows(const gg_agg *agg, const ggp_aggmap *aggmap, const gg
 {
 	if (n == 0 && agg->numCols == 0 && !empty_is_empty) { recs.resize(1); memset(&recs[0], 0, sizeof(ggp_grec)); n = 1; }
 	if (n > outcap) { gg_set_error("output capacity %d < %lld groups", outcap, n); return GG_ERR_NOMEM; }
-	finalize_rows(agg, aggmap, prog, final_stage, recs.data(), (int) n, out);
+	const int rc = finalize_rows(agg, aggmap, prog, final_stage, recs.data(), (int) n, out);
+	if (rc) return rc;
 	*nout = (int) n;
 	return GG_OK;
 }
@@ -908,6 +914,11 @@ int gg_scanagg_fetch(gg_scanagg *p, gg_aggrow *out, int outcap, int *nout,
 	uint32_t flags = p->h_mirror->st.err;
 	unsigned long long counters[2] = { p->h_mirror->st.counters[0], p->h_mirror->st.counters[1] };
 	int n = p->h_mirror->st.nout;
+	if (p->build_err)
+	{
+		const int brc = gg_errflags_to_code(p->build_err);        /* the join's hash table holds a value the device refused */
+		if (brc) return brc;
+	}
 	/* Escalation, then the inputs are replayed and fetched again.  Private accumulators: more groups than they hold (the
 	 * planner's numGroups was low or absent), or a non-finite private sum, which only the value-tracking transposed variant can
 	 * attribute to an infinite input or to a float8pl overflow.  A block-table variant with more groups than a block holds:

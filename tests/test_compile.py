@@ -92,6 +92,38 @@ def test_join_programs_shape():
     assert not any("off=" in ln and "idx=12" in ln and "off=-1" not in ln for ln in probe)   # no tuple offsets for payload reads
 
 
+def test_join_carries_inner_numeric_columns_as_scaled_integers():
+    """An inner numeric column above a join travels in the hash-table payload as its scaled 64-bit integer: the build program
+    decodes it (LD_NUM at the column's declared scale, the scale shown as cc=) into an OUT slot, and the probe program reads
+    the payload slot (idx >= 128), rescaled by a multiply where the expression needs a larger scale."""
+    import _numeric as nref
+    NUM = capi.NUMERICOID
+    odesc = capi.gg_tupdesc()
+    idesc = capi.gg_tupdesc()
+    for d, spec in ((odesc, [(capi.INT4OID, -1), (NUM, nref.typmod(18, 4))]), (idesc, [(capi.INT4OID, -1), (NUM, nref.typmod(15, 2)), (NUM, nref.typmod(12, 0))])):
+        d.natts = len(spec)
+        for i, (t, tm) in enumerate(spec):
+            a = d.attrs[i]
+            a.atttypid, a.attlen, a.attalign, a.attbyval, a.atttypmod, a.attnotnull = t, 4 if t == capi.INT4OID else -1, ord("i"), int(t == capi.INT4OID), tm, 1
+    p = ExprPool()
+    ok, ik = p.var(1, capi.INT4OID, 0), p.var(1, capi.INT4OID, 1)
+    x, y, z = p.var(2, NUM, 0), p.var(2, NUM, 1), p.var(3, NUM, 1)
+    qual = p.func(capi.F_NUMERIC_LT, capi.BOOLOID, x, y)                        # outer scale 4 < inner scale 2: inner rescaled x100
+    hj = capi.make_hashjoin(capi.JOIN_INNER, [ok], [ik], qual)
+    agg = capi.make_agg(capi.AGGSTAGE_NORMAL, [], [(capi.AGG_SUM_NUMERIC, y), (capi.AGG_SUM_NUMERIC, p.func(capi.F_NUMERIC_MUL, NUM, x, z))])
+    build, probe, text = disasm_join(capi.make_scan(odesc, -1), capi.make_scan(idesc, -1), hj, agg, p.pool)
+    ops = [ln.split() for ln in build]
+    outs = [ln for ln in build if " OUT" in ln]
+    assert len(outs) == 2 and all(ln.split()[1] == "LD_NUM" for ln in outs), build
+    assert sorted(ln.split()[3] for ln in outs) == ["cc=0", "cc=2"], build       # each at its own column's scale
+    assert not any(o[1] == "LD_BOOL" for o in ops), build
+    inner_loads = [ln for ln in probe if ln.split()[1] == "LD_NUM" and int(ln.split()[2][4:]) >= 128]
+    assert len(inner_loads) >= 3, probe                                          # qual, sum(y), x * z
+    assert all("off=-1" in ln for ln in inner_loads), probe                       # from the payload, not from a tuple offset
+    nxt = [probe[probe.index(ln) + 1].split()[1] for ln in inner_loads if "cc=2" in ln]
+    assert "IMUL_K" in nxt, probe                                                 # y at scale 4 for the comparison
+
+
 def test_join_shapes_outside_the_subset_are_refused():
     outer, inner, hj, agg, pool = tpch.join_plan(kind="count")
     hj.jointype = 7                                                          # JOIN_UNIQUE_OUTER (planner-internal)

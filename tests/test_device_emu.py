@@ -519,6 +519,93 @@ def test_numeric_finalisation_equals_the_references_sum_and_avg():
             assert capi.numeric_of_aggval(v) == case[name], (name, capi.numeric_of_aggval(v), case[name])
 
 
+def test_exact_numeric_reference_restates_the_references_sum_and_avg():
+    """tests/_numeric.py (the exact reference the GPU numeric tests compare with) against numeric_kat.json's sums and
+    averages, which the reference's own numeric.o computed: every digit and the display scale"""
+    import json
+    import _numeric as nref
+    kat = json.load(open(os.path.join(HERE, "golden", "numeric_kat.json")))
+    for case in kat["sumavg"]:
+        parsed = [capi.numeric_parse(t) for t in case["values"]]
+        sc = max(s for _, s in parsed)
+        vals = [nref.rescale(v, s, sc) for v, s in parsed]
+        assert nref.sum_text(vals, sc) == case["sum"]
+        assert nref.avg_text(vals, sc) == case["avg"], (case["avg"], nref.avg_text(vals, sc))
+    assert len(kat["sumavg"]) >= 60
+
+
+def _numeric_sum_through_the_interpreter(emu, values, scale, precision=38):
+    """sum(x) over rows of one numeric(precision, scale) column through the product's compiler + interpreter (host build):
+    (error flags, the sum at `scale` or None)"""
+    import _numeric as nref
+    desc = capi.gg_tupdesc()
+    desc.natts = 1
+    a = desc.attrs[0]
+    a.atttypid, a.attlen, a.attalign, a.attbyval, a.atttypmod, a.attnotnull = capi.NUMERICOID, -1, ord("i"), 0, nref.typmod(precision, scale), 1
+    pages = po.build_pages(desc, [[capi.numeric_payload(v, scale)] for v in values])
+    p = ExprPool()
+    agg = capi.make_agg(capi.AGGSTAGE_NORMAL, [], [(capi.AGG_SUM_NUMERIC, p.var(1, capi.NUMERICOID))])
+    groups, aggcol, sc, ps, err = run_emu(emu, capi.make_scan(desc, -1), agg, p.pool, pages)
+    assert sc == len(values) and len(groups) == 1
+    col = aggcol[0]
+    lo, hi = int(np.float64(groups[0].sum[col]).view(np.int64)), int(np.float64(groups[0].sum[col + 1]).view(np.int64))
+    return err, hi * 2 ** 32 + lo
+
+
+# the leading five base-10000 digits form an integer in [2^64, 2^64 + 8383]: v * 10000 + digit carries past 2^64
+WRAP_FAMILY = [
+    ([2 ** 64 + 1, 3], 0, 20),                              # the sum came back as 4
+    ([2 ** 64 + 7, 3], 4, 20),                              # 1844674407370955.1623 + 0.0003 came back as 0.0010
+    ([-(2 ** 64 + 2792) * 10 ** 4], 0, 24),                 # -184467440737095544080000 came back as -27920000
+    ([(2 ** 64 + 8383) * 10 ** 4, 1], 4, 24),               # an integer at scale 4: its digits align with 10^(4k) all the same
+    ([2 ** 64, -5], 0, 20), ([-(2 ** 64 + 100)], 8, 28), ([(2 ** 64 + 4000) * 10 ** 8], 8, 36),
+]
+
+
+def test_numeric_decoder_refuses_values_whose_digits_carry_past_2_64(emu):
+    """The 2^64 wrap family through the interpreter must raise GGP_EF_NUMERIC_RANGE: every such value is >= 2^63 at its
+    column scale, so no answer is right but a refusal.  With the carry of the last digit unchecked, the decoder wrapped to a
+    small number and the sums above came back wrong without an error flag."""
+    for values, scale, prec in WRAP_FAMILY:
+        err, got = _numeric_sum_through_the_interpreter(emu, values, scale, prec)
+        assert err & 0x8000, (values, scale, got)
+
+
+def test_numeric_sums_near_the_64_bit_edges_are_exact_or_refused(emu):
+    """Seeded pairs of values near 10^k, 2^63 and 2^64 (times 10^(4j), so that the base-10000 digits line up with the carry)
+    at scales 0, 2, 4, 8 and 15: the interpreter's sum equals the exact one, or it is refused — a refusal when an input is >= 2^63
+    at its scale, and an exact answer when every input is below 2^62."""
+    import _numeric as nref
+    rng = np.random.default_rng(64)
+    stats = {nref.REQUIRED: 0, nref.FORBIDDEN: 0, nref.EITHER: 0, "refused": 0}
+    for trial in range(300):
+        scale = int(rng.choice([0, 2, 4, 8, 15]))
+        vals = []
+        for _ in range(2):
+            kind = int(rng.integers(0, 4))
+            if kind <= 1:
+                base = 10 ** int(rng.integers(0, 27))
+            elif kind == 2:
+                base = 2 ** 63
+            else:
+                base = 2 ** 64 * 10 ** (4 * int(rng.integers(0, 3)))
+            v = base + int(rng.integers(-9000, 9000))
+            vals.append(v if rng.random() < 0.5 else -v)
+        rule = nref.refusal(vals, [])
+        stats[rule] += 1
+        err, got = _numeric_sum_through_the_interpreter(emu, vals, scale)
+        refused = bool(err & 0x8000)
+        stats["refused"] += refused
+        assert not (err & ~0x8000), (trial, hex(err))
+        if rule == nref.REQUIRED:
+            assert refused, (trial, vals, scale, got)
+        elif rule == nref.FORBIDDEN:
+            assert not refused and got == sum(vals), (trial, vals, scale, got)
+        elif not refused:
+            assert got == sum(vals), (trial, vals, scale, got)
+    assert stats[nref.REQUIRED] > 100 and stats[nref.FORBIDDEN] > 20, stats
+
+
 def test_random_numeric_expressions_mean_what_the_oracle_computes(emu):
     """numeric_add / _sub / _mul trees, comparisons in the qual, NULLs, columns of different scales: sums (both halves) and
     counts of the device interpreter equal the oracle's exact sums"""
