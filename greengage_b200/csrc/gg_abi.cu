@@ -109,7 +109,6 @@ void gg_engine_free(gg_engine *e)
 	cudaSetDevice(e->device);
 	cudaStreamSynchronize(e->stream);
 	cudaStreamSynchronize(e->copy_stream);
-	cudaFree(e->final_scratch);
 	cudaFree(e->sort_scratch);
 	cudaFree(e->motion_state);
 	cudaFree(e->snapshot_buf);

@@ -718,30 +718,17 @@ static void compile_agg_part(Ctx &c, const gg_agg *agg, ggp_aggmap *aggmap)
 	for (int i = 0; i < agg->numAggs && !c.failed; i++)
 	{
 		const gg_aggref &ar = agg->aggs[i];
-		int kind = 0, sq = 0;
-		bool isnum = false;
+		const int kind = ggp_acckind_of(ar.aggfnoid);
 		aggmap[i].scale = 0;
-		switch (ar.aggfnoid)
-		{
-			case GG_AGG_COUNT_STAR: aggmap[i].col = -1; continue;
-			case GG_AGG_COUNT_ANY: kind = GGP_ACC_COUNT; break;
-			case GG_AGG_SUM_FLOAT8: kind = GGP_ACC_F8SUM; break;
-			/* float8_accum also maintains sumX2, which float8_avg ignores (float.c:1982): only a PARTIAL stage,
-			 * whose transition state {N, sumX, sumX2} is shipped to another process, has to produce it */
-			case GG_AGG_AVG_FLOAT8: kind = GGP_ACC_F8SUM; sq = (agg->aggstage == GG_AGGSTAGE_PARTIAL) && !(agg->flags & GG_AGGF_DEVICE_FINAL); break;
-			case GG_AGG_MIN_FLOAT8: kind = GGP_ACC_F8MIN; break;
-			case GG_AGG_MAX_FLOAT8: kind = GGP_ACC_F8MAX; break;
-			case GG_AGG_SUM_INT4: kind = GGP_ACC_I8SUM; break;
-			case GG_AGG_SUM_NUMERIC: case GG_AGG_AVG_NUMERIC:
-				/* numeric_avg_accum (numeric.c:3057): N and an exact running sum — here a 128-bit integer at the argument's
-				 * scale, kept as two int64 sums of the inputs' halves */
-				kind = GGP_ACC_I8SUM; isnum = true;
-				if (agg->aggstage != GG_AGGSTAGE_NORMAL) fail(c, "numeric aggregates run as one-stage aggregates on the GPU path");
-				break;
-			case GG_AGG_MIN_INT4: case GG_AGG_MIN_INT8: case GG_AGG_MIN_DATE: kind = GGP_ACC_I8MIN; break;
-			case GG_AGG_MAX_INT4: case GG_AGG_MAX_INT8: case GG_AGG_MAX_DATE: kind = GGP_ACC_I8MAX; break;
-			default: fail(c, "aggregate %d not supported on the GPU path", ar.aggfnoid); continue;
-		}
+		if (kind < 0) { fail(c, "aggregate %d not supported on the GPU path", ar.aggfnoid); continue; }
+		if (kind == 0) { aggmap[i].col = -1; continue; }              /* count(*) */
+		/* float8_accum also maintains sumX2, which float8_avg ignores (float.c:1982): only a PARTIAL stage,
+		 * whose transition state {N, sumX, sumX2} is shipped to another process, has to produce it */
+		const int sq = ar.aggfnoid == GG_AGG_AVG_FLOAT8 && agg->aggstage == GG_AGGSTAGE_PARTIAL && !(agg->flags & GG_AGGF_DEVICE_FINAL);
+		/* numeric_avg_accum (numeric.c:3057): N and an exact running sum — here a 128-bit integer at the argument's
+		 * scale, kept as two int64 sums of the inputs' halves */
+		const bool isnum = ar.aggfnoid == GG_AGG_SUM_NUMERIC || ar.aggfnoid == GG_AGG_AVG_NUMERIC;
+		if (isnum && agg->aggstage != GG_AGGSTAGE_NORMAL) fail(c, "numeric aggregates run as one-stage aggregates on the GPU path");
 		if (ar.arg < 0) { fail(c, "aggregate %d needs an argument", ar.aggfnoid); continue; }
 		int found = -1;
 		for (int j = 0; j < prog->nacc; j++)

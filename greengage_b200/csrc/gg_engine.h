@@ -19,8 +19,6 @@ struct gg_engine {
 	cudaEvent_t ev_t0 = nullptr, ev_t1 = nullptr;      /* gg_engine_timer_start/stop */
 	bool timed = false;
 	uint64_t launches = 0;
-	void *final_scratch = nullptr;       /* gg_agg_final: device scratch kept across calls, grown on demand */
-	size_t final_cap = 0;                /* records it holds */
 	void *sort_scratch = nullptr;        /* gg_sort_*: key/value ping-pong buffers, histograms; kept across calls */
 	size_t sort_scratch_bytes = 0;
 	std::vector<void *> groups_pool;     /* gg_groups buffers of the common size, recycled (gg_scanagg.cu) */

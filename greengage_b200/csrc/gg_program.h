@@ -204,6 +204,24 @@ struct ggp_aggmap {          /* how each Aggref reads the accumulator columns */
 	int32_t col;             /* accumulator column, -1 for count(*); numeric sum / avg: the low half, col + 1 the high half */
 	int32_t scale;           /* numeric sum / avg: display scale of the summed expression */
 };
+/* the accumulator column an aggregate's transition state lives in (ggp_acckind); 0 for count(*), whose state is
+ * ggp_grec::count and needs no column; -1 for an aggregate the device does not run */
+static inline int ggp_acckind_of(int32_t aggfnoid)
+{
+	switch (aggfnoid)
+	{
+		case GG_AGG_COUNT_STAR: return 0;
+		case GG_AGG_COUNT_ANY: return GGP_ACC_COUNT;
+		case GG_AGG_SUM_FLOAT8: case GG_AGG_AVG_FLOAT8: return GGP_ACC_F8SUM;
+		case GG_AGG_MIN_FLOAT8: return GGP_ACC_F8MIN;
+		case GG_AGG_MAX_FLOAT8: return GGP_ACC_F8MAX;
+		/* numeric: a 128-bit integer sum kept as two int64 sums of the inputs' halves (col, col + 1) */
+		case GG_AGG_SUM_INT4: case GG_AGG_SUM_NUMERIC: case GG_AGG_AVG_NUMERIC: return GGP_ACC_I8SUM;
+		case GG_AGG_MIN_INT4: case GG_AGG_MIN_INT8: case GG_AGG_MIN_DATE: return GGP_ACC_I8MIN;
+		case GG_AGG_MAX_INT4: case GG_AGG_MAX_INT8: case GG_AGG_MAX_DATE: return GGP_ACC_I8MAX;
+		default: return -1;
+	}
+}
 int ggp_compile_scanagg(const gg_scan *scan, const gg_agg *agg, const gg_exprpool *pool,
                         ggp_program *prog, ggp_aggmap *aggmap, char *err, int errlen);
 int ggp_disasm(const ggp_program *p, char *buf, int cap);

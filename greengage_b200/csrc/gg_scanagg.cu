@@ -769,8 +769,7 @@ extern "C" int gg_debug_numeric_final(int which, int64_t lo, int64_t hi, int sca
 	return 0;
 }
 
-static int finalize_rows(const gg_agg *agg, const ggp_aggmap *aggmap, const ggp_program *prog, int final_stage,
-                         const ggp_grec *recs, int n, gg_aggrow *out)
+static int finalize_rows(const gg_agg *agg, const ggp_aggmap *aggmap, const uint8_t *keytype, const ggp_grec *recs, int n, gg_aggrow *out)
 {
 	for (int g = 0; g < n; g++)
 	{
@@ -781,7 +780,7 @@ static int finalize_rows(const gg_agg *agg, const ggp_aggmap *aggmap, const ggp_
 		{
 			row.keyisnull[c] = (x.keynull >> c) & 1;
 			row.key[c] = (int64_t) x.key[c];
-			if (prog->keytype[c] == 3 && !row.keyisnull[c])
+			if (keytype[c] == 3 && !row.keyisnull[c])
 			{
 				int len = 0;
 				while (len < 8 && ((x.key[c] >> (8 * len)) & 0xff)) len++;
@@ -805,10 +804,7 @@ static int finalize_rows(const gg_agg *agg, const ggp_aggmap *aggmap, const ggp_
 			switch (fn)
 			{
 				case GG_AGG_COUNT_ANY:
-					v.i = final_stage ? ibits : (int64_t) nn;
-					break;
-				case GG_AGG_COUNT_STAR:       /* FINAL stage only: int8pl over partial counts */
-					v.i = ibits;
+					v.i = (int64_t) nn;
 					break;
 				case GG_AGG_SUM_FLOAT8:
 				case GG_AGG_MIN_FLOAT8:
@@ -861,12 +857,12 @@ static int finalize_rows(const gg_agg *agg, const ggp_aggmap *aggmap, const ggp_
 
 /* merged group records -> rows (finalize_aggregate, nodeAgg.c:871-999).  Plain aggregation over zero rows still yields one row
  * (nodeAgg.c:1247-1400), unless `empty_is_empty` (a segment that does not own the result). */
-static int records_to_rows(const gg_agg *agg, const ggp_aggmap *aggmap, const ggp_program *prog, int final_stage, std::vector<ggp_grec> &recs,
+static int records_to_rows(const gg_agg *agg, const ggp_aggmap *aggmap, const uint8_t *keytype, std::vector<ggp_grec> &recs,
                            long long n, bool empty_is_empty, gg_aggrow *out, int outcap, int *nout)
 {
 	if (n == 0 && agg->numCols == 0 && !empty_is_empty) { recs.resize(1); memset(&recs[0], 0, sizeof(ggp_grec)); n = 1; }
 	if (n > outcap) { gg_set_error("output capacity %d < %lld groups", outcap, n); return GG_ERR_NOMEM; }
-	const int rc = finalize_rows(agg, aggmap, prog, final_stage, recs.data(), (int) n, out);
+	const int rc = finalize_rows(agg, aggmap, keytype, recs.data(), (int) n, out);
 	if (rc) return rc;
 	*nout = (int) n;
 	return GG_OK;
@@ -966,7 +962,7 @@ int gg_scanagg_fetch(gg_scanagg *p, gg_aggrow *out, int outcap, int *nout,
 		}
 		int rc = gg_errflags_to_code(flags & ~(uint32_t) GGP_EF_GROUP_OVERFLOW);
 		if (rc) return rc;
-		return records_to_rows(&p->agg, p->aggmap, &p->prog, 0, recs, (long long) n64, false, out, outcap, nout);
+		return records_to_rows(&p->agg, p->aggmap, p->prog.keytype, recs, (long long) n64, false, out, outcap, nout);
 	}
 	int rc = gg_errflags_to_code(flags);
 	if (rc) return rc;
@@ -974,7 +970,7 @@ int gg_scanagg_fetch(gg_scanagg *p, gg_aggrow *out, int outcap, int *nout,
 	recs.resize((size_t) (n > 0 ? n : 0));
 	if (n > 0 && n <= GGP_FAST_GROUPS) memcpy(recs.data(), p->h_mirror->recs, sizeof(ggp_grec) * (size_t) n);     /* already here */
 	else if (n > 0) GG_CUDA(cudaMemcpy(recs.data(), p->recs, sizeof(ggp_grec) * n, cudaMemcpyDeviceToHost));
-	return records_to_rows(&p->agg, p->aggmap, &p->prog, 0, recs, n, false, out, outcap, nout);
+	return records_to_rows(&p->agg, p->aggmap, p->prog.keytype, recs, n, false, out, outcap, nout);
 }
 
 int gg_scanagg_scan_kernel_ms(gg_scanagg *p, float *ms, int *launches)
@@ -1017,9 +1013,9 @@ void gg_scanagg_free(gg_scanagg *p)
 	delete p;
 }
 
-/* FINAL-stage Agg: the partial rows of all segments become group records (one accumulator column per
- * aggregate) and go through the same deterministic merge kernel; combine functions float8pl /
- * float8_combine / int8pl (nodeAgg.c:2123-2148, float.c:1842, int8.c:513). */
+/* FINAL-stage Agg over partial rows on the host: the rows become group records laid out as a PARTIAL pipeline leaves them on
+ * the device, and gg_groups_final combines them (float8pl / float8_combine / int8pl, nodeAgg.c:2123-2148, float.c:1842,
+ * int8.c:513). */
 int gg_agg_final(gg_engine *e, const gg_agg *agg, const gg_aggrow *in, int nin,
                  gg_aggrow *out, int outcap, int *nout)
 {
@@ -1028,39 +1024,26 @@ int gg_agg_final(gg_engine *e, const gg_agg *agg, const gg_aggrow *in, int nin,
 	{ gg_set_error("gg_agg_final: %d grouping columns, %d aggregates, %d rows in, room for %d", agg->numCols, agg->numAggs, nin, outcap); return GG_ERR_ARG; }
 	if (agg->numAggs > GGP_MAX_ACCS) { gg_set_error("too many aggregates"); return GG_ERR_UNSUPPORTED; }
 	GG_CUDA(cudaSetDevice(e->device));
-	ggp_program prog;
-	ggp_aggmap aggmap[GG_MAX_AGGS];
-	ggp_acckinds kinds;
-	memset(&prog, 0, sizeof prog);
-	memset(&kinds, 0, sizeof kinds);
-	prog.nkeys = agg->numCols;
-	prog.nacc = agg->numAggs;
+	gg_groups like = gg_groups();
+	like.agg = *agg;
+	like.nkeys = agg->numCols;
 	for (int c = 0; c < agg->numCols; c++)
 	{
-		int32_t t = agg->grpCol[c];
-		prog.keytype[c] = (t == GG_FLOAT8OID) ? 2 : (t == GG_BPCHAROID || t == GG_VARCHAROID || t == GG_TEXTOID) ? 3 : 1;
+		int32_t t = agg->grpCol[c];                    /* a FINAL Agg's grpCol carries the key type OIDs */
+		like.keytype[c] = (t == GG_FLOAT8OID) ? 2 : (t == GG_BPCHAROID || t == GG_VARCHAROID || t == GG_TEXTOID) ? 3 : 1;
 	}
 	for (int i = 0; i < agg->numAggs; i++)
 	{
-		aggmap[i].col = i;
-		switch (agg->aggs[i].aggfnoid)
-		{
-			case GG_AGG_COUNT_STAR: case GG_AGG_COUNT_ANY: case GG_AGG_SUM_INT4: kinds.k[i] = GGP_ACC_I8SUM; break;
-			case GG_AGG_SUM_FLOAT8: case GG_AGG_AVG_FLOAT8: kinds.k[i] = GGP_ACC_F8SUM; break;
-			case GG_AGG_MIN_FLOAT8: kinds.k[i] = GGP_ACC_F8MIN; break;
-			case GG_AGG_MAX_FLOAT8: kinds.k[i] = GGP_ACC_F8MAX; break;
-			case GG_AGG_MIN_INT4: case GG_AGG_MIN_INT8: case GG_AGG_MIN_DATE: kinds.k[i] = GGP_ACC_I8MIN; break;
-			case GG_AGG_MAX_INT4: case GG_AGG_MAX_INT8: case GG_AGG_MAX_DATE: kinds.k[i] = GGP_ACC_I8MAX; break;
-			default: gg_set_error("aggregate %d not supported", agg->aggs[i].aggfnoid); return GG_ERR_UNSUPPORTED;
-		}
-		prog.acckind[i] = kinds.k[i];
+		const int fn = agg->aggs[i].aggfnoid, kind = ggp_acckind_of(fn);
+		if (kind < 0 || fn == GG_AGG_SUM_NUMERIC || fn == GG_AGG_AVG_NUMERIC) { gg_set_error("aggregate %d not supported", fn); return GG_ERR_UNSUPPORTED; }
+		like.aggmap[i].col = kind ? like.nacc : -1;
+		if (kind) like.acckind[like.nacc++] = (uint8_t) kind;
 	}
-	std::vector<ggp_grec> recs((size_t) (nin > 0 ? nin : 1));
+	std::vector<ggp_grec> recs((size_t) nin);
 	uint32_t hostflags = 0;
 	for (int r = 0; r < nin; r++)
 	{
 		ggp_grec &x = recs[r];
-		memset(&x, 0, sizeof x);
 		x.valid = 1;
 		for (int c = 0; c < agg->numCols; c++)
 		{
@@ -1068,7 +1051,7 @@ int gg_agg_final(gg_engine *e, const gg_agg *agg, const gg_aggrow *in, int nin,
 			else
 			{
 				uint64_t k = (uint64_t) in[r].key[c];
-				if (prog.keytype[c] == 2)
+				if (like.keytype[c] == 2)
 				{
 					double d; memcpy(&d, &k, 8);
 					if (d == 0.0) k = 0; else if (d != d) k = 0x7ff8000000000000ull;
@@ -1081,59 +1064,42 @@ int gg_agg_final(gg_engine *e, const gg_agg *agg, const gg_aggrow *in, int nin,
 		for (int i = 0; i < agg->numAggs; i++)
 		{
 			const gg_aggval &v = in[r].agg[i];
+			const int j = like.aggmap[i].col;
 			switch (agg->aggs[i].aggfnoid)
 			{
+				case GG_AGG_COUNT_STAR:
+					x.count = v.isnull ? 0 : (uint64_t) v.i;
+					break;
+				case GG_AGG_COUNT_ANY:
+					x.n[j] = v.isnull ? 0 : (uint64_t) v.i;
+					break;
 				case GG_AGG_AVG_FLOAT8:
-					x.n[i] = (uint64_t) v.f[0]; x.sum[i] = v.f[1]; x.sumsq[i] = v.f[2];
+					x.n[j] = (uint64_t) v.f[0]; x.sum[j] = v.f[1]; x.sumsq[j] = v.f[2];
 					if (!(fabs(v.f[1]) < INFINITY) || !(fabs(v.f[2]) < INFINITY)) hostflags |= GGP_EF_SAW_INF;
 					/* float8_combine adds N even when it is 0; a zero-N state contributes nothing */
 					break;
 				case GG_AGG_SUM_FLOAT8: case GG_AGG_MIN_FLOAT8: case GG_AGG_MAX_FLOAT8:
-					x.n[i] = v.isnull ? 0 : 1; x.sum[i] = v.f[0];
+					x.n[j] = v.isnull ? 0 : 1; x.sum[j] = v.f[0];
 					if (!v.isnull && !(fabs(v.f[0]) < INFINITY)) hostflags |= GGP_EF_SAW_INF;
 					break;
 				default:
-					x.n[i] = v.isnull ? 0 : 1; memcpy(&x.sum[i], &v.i, 8);
+					x.n[j] = v.isnull ? 0 : 1; memcpy(&x.sum[j], &v.i, 8);
 					break;
 			}
 		}
 	}
-	int n = 0;
-	uint32_t flags = 0;
-	const int cap = nin > 0 ? nin : 1;
-	/* one scratch allocation kept in the engine: [recs cap][out cap][vidx cap][vmap cap][n][err] */
-	if (e->final_cap < (size_t) cap)
-	{
-		size_t want = (size_t) cap < 256 ? 256 : (size_t) cap;
-		cudaFree(e->final_scratch);
-		e->final_scratch = nullptr; e->final_cap = 0;
-		GG_CUDA(cudaMalloc(&e->final_scratch, want * (2 * sizeof(ggp_grec) + 2 * sizeof(int)) + 64));
-		e->final_cap = want;
-	}
-	ggp_grec *d_recs = (ggp_grec *) e->final_scratch;
-	ggp_grec *d_out = d_recs + e->final_cap;
-	int *d_vidx = (int *) (d_out + e->final_cap);
-	int *d_vmap = d_vidx + e->final_cap;
-	int *d_n = d_vmap + e->final_cap;
-	uint32_t *d_err = (uint32_t *) (d_n + 1);
-	GG_CUDA(cudaMemcpyAsync(d_recs, recs.data(), sizeof(ggp_grec) * (size_t) nin, cudaMemcpyHostToDevice, e->stream));
-	GG_CUDA(cudaMemcpyAsync(d_err, &hostflags, sizeof hostflags, cudaMemcpyHostToDevice, e->stream));
-	GG_CUDA(cudaMemsetAsync(d_out, 0, sizeof(ggp_grec) * cap, e->stream));
-	gg_merge_recs_kernel<<<1, 1024, 0, e->stream>>>(d_recs, nin, agg->numCols, agg->numAggs, kinds,
-	                                               d_out, cap, d_n, d_vidx, d_vmap, d_err, 1);
-	cudaError_t le = cudaGetLastError();
-	e->launches++;
-	if (le == cudaSuccess) le = cudaMemcpyAsync(&n, d_n, sizeof n, cudaMemcpyDeviceToHost, e->stream);
-	if (le == cudaSuccess) le = cudaMemcpyAsync(&flags, d_err, sizeof flags, cudaMemcpyDeviceToHost, e->stream);
-	if (le == cudaSuccess) le = cudaStreamSynchronize(e->stream);
-	std::vector<ggp_grec> merged((size_t) (n > 0 ? n : 0));
-	if (le == cudaSuccess && n > 0) le = cudaMemcpy(merged.data(), d_out, sizeof(ggp_grec) * n, cudaMemcpyDeviceToHost);
-	if (le != cudaSuccess) return gg_cuda_fail(le, "gg_agg_final");
-	int rc = gg_errflags_to_code(flags);
-	if (rc) return rc;
-	gg_agg fin = *agg;
-	fin.aggstage = GG_AGGSTAGE_FINAL;
-	return records_to_rows(&fin, aggmap, &prog, 1, merged, n, false, out, outcap, nout);
+	gg_groups *g = gg_groups_alloc(e, &like, nin, false);
+	if (!g) return GG_ERR_NOMEM;
+	/* GGP_EF_SAW_INF lets the merge tell an infinite partial sum from a float8pl overflow */
+	const gg_groupstatus st = { hostflags, nin, { 0, 0 } };
+	cudaError_t ce = nin ? cudaMemcpyAsync(g->recs, recs.data(), sizeof(ggp_grec) * (size_t) nin, cudaMemcpyHostToDevice, e->stream) : cudaSuccess;
+	if (ce == cudaSuccess) ce = cudaMemcpyAsync(g->d_status, &st, sizeof st, cudaMemcpyHostToDevice, e->stream);
+	gg_groups *fin = nullptr;
+	int rc = ce != cudaSuccess ? gg_cuda_fail(ce, "gg_agg_final") : gg_groups_final(e, g, &fin);
+	if (rc == GG_OK) rc = gg_groups_fetch(fin, out, outcap, nout, nullptr, nullptr);
+	gg_groups_free(fin);
+	gg_groups_free(g);
+	return rc;
 }
 
 
@@ -1205,14 +1171,16 @@ int gg_scanagg_groups(gg_scanagg *p, gg_groups **out)
 	return GG_OK;
 }
 
-/* FINAL-stage Agg on the device: combine the records a Motion delivered (float8pl / float8_combine / int8pl,
- * nodeAgg.c:2123-2148) with the deterministic merge kernel; the result reads like a one-stage aggregate's. */
+/* FINAL-stage Agg on the device: combine partial group records — what a Motion delivered, a pipeline's result or the rows
+ * gg_agg_final was given (float8pl / float8_combine / int8pl, nodeAgg.c:2123-2148) — with the deterministic merge kernel; the
+ * result reads like a one-stage aggregate's. */
 int gg_groups_final(gg_engine *e, gg_groups *in, gg_groups **out)
 {
 	if (!e || !in || !out) return GG_ERR_ARG;
 	*out = nullptr;
 	GG_CUDA(cudaSetDevice(e->device));
-	const int cap = in->cap < GG_GROUPS_POOL_CAP ? in->cap : (in->sparse ? in->cap : GG_GROUPS_POOL_CAP);
+	/* every valid record of the input may be a group of its own, so the output has the input's size */
+	const int cap = in->cap;
 	gg_groups *g = gg_groups_alloc(e, in, cap, false);
 	if (!g) return GG_ERR_NOMEM;
 	g->agg.aggstage = GG_AGGSTAGE_NORMAL;          /* combined states finalise like a one-stage aggregate's (float8_avg = sumX / N) */
@@ -1223,8 +1191,7 @@ int gg_groups_final(gg_engine *e, gg_groups *in, gg_groups **out)
 	if (ce == cudaSuccess) ce = cudaMemsetAsync(g->recs, 0, sizeof(ggp_grec) * (size_t) cap, st);
 	if (ce == cudaSuccess)
 	{
-		const int nrecs = in->sparse ? in->cap : (in->cap < GG_GROUPS_POOL_CAP ? in->cap : GG_GROUPS_POOL_CAP);
-		gg_merge_recs_kernel<<<1, 1024, 0, st>>>(in->recs, nrecs, in->nkeys, in->nacc, kinds, g->recs, cap, g->d_n,
+		gg_merge_recs_kernel<<<1, 1024, 0, st>>>(in->recs, cap, in->nkeys, in->nacc, kinds, g->recs, cap, g->d_n,
 		                                        g->scratch, g->scratch + g->alloc_cap, &g->d_status->err, in->sparse ? 0 : 1);
 		ce = cudaGetLastError();
 		e->launches++;
@@ -1274,10 +1241,7 @@ int gg_groups_fetch(gg_groups *g, gg_aggrow *out, int outcap, int *nout, uint64_
 		if (n > 0 && n <= first) memcpy(recs.data(), hr, sizeof(ggp_grec) * (size_t) n);
 		else if (n > 0) GG_CUDA(cudaMemcpy(recs.data(), g->recs, sizeof(ggp_grec) * (size_t) n, cudaMemcpyDeviceToHost));
 	}
-	std::vector<ggp_program> pb(1);
-	memset(&pb[0], 0, sizeof(ggp_program));
-	memcpy(pb[0].keytype, g->keytype, sizeof g->keytype);
-	return records_to_rows(&g->agg, g->aggmap, &pb[0], 0, recs, (long long) recs.size(), g->empty_is_empty, out, outcap, nout);
+	return records_to_rows(&g->agg, g->aggmap, g->keytype, recs, (long long) recs.size(), g->empty_is_empty, out, outcap, nout);
 }
 
 int gg_groups_info(gg_groups *g, int *sparse, int *cap)

@@ -528,6 +528,154 @@ def test_final_stage_combine(eng):
     assert agg_final(eng, fin, []) == []
 
 
+# a FINAL Agg over partial rows made by hand: one int4 key (grpCol carries its type OID) and every combinable aggregate
+FINAL_AGGS = [capi.AGG_COUNT_STAR, capi.AGG_COUNT_ANY, capi.AGG_SUM_INT4, capi.AGG_MIN_INT4, capi.AGG_MAX_INT4, capi.AGG_MIN_INT8,
+              capi.AGG_MAX_INT8, capi.AGG_MIN_DATE, capi.AGG_MAX_DATE, capi.AGG_MIN_FLOAT8, capi.AGG_MAX_FLOAT8, capi.AGG_SUM_FLOAT8,
+              capi.AGG_AVG_FLOAT8]
+
+
+def _final_agg(aggs=FINAL_AGGS, keys=(capi.INT4OID,)):
+    return capi.make_agg(capi.AGGSTAGE_FINAL, list(keys), [(fn, 0) for fn in aggs])
+
+
+def _partial_rows(keys, per_key, seed, null_rate=0.3):
+    """per_key partial rows of FINAL_AGGS for every key (None: the NULL key), shuffled.  Float8 values are multiples of 1/4
+    below 2^20, so every summation order gives the same bits; NULL partial states appear where a segment saw no input."""
+    rng = np.random.default_rng(seed)
+    rows = []
+    for k in keys:
+        for _ in range(per_key):
+            r = capi.gg_aggrow()
+            if k is None:
+                r.keyisnull[0] = 1
+            else:
+                r.key[0] = k
+            n = int(rng.integers(0, 5))
+            nx = 0 if rng.random() < null_rate else int(rng.integers(1, n + 2))
+            r.agg[0].i, r.agg[1].i = n, nx
+            for i, fn in enumerate(FINAL_AGGS[2:], 2):
+                v = r.agg[i]
+                if fn == capi.AGG_AVG_FLOAT8:
+                    s = float(rng.integers(-4000, 4000)) / 4
+                    v.f[0], v.f[1], v.f[2] = nx, s if nx else 0.0, s * s / 4 if nx else 0.0
+                elif not nx:
+                    v.isnull = 1
+                elif fn in (capi.AGG_MIN_FLOAT8, capi.AGG_MAX_FLOAT8, capi.AGG_SUM_FLOAT8):
+                    v.f[0] = float(rng.integers(-4000, 4000)) / 4
+                elif fn in (capi.AGG_MIN_INT8, capi.AGG_MAX_INT8):
+                    v.i = int(rng.integers(-2 ** 62, 2 ** 62))
+                elif fn in (capi.AGG_MIN_DATE, capi.AGG_MAX_DATE):
+                    v.i = int(rng.integers(-30000, 30000))
+                else:
+                    v.i = int(rng.integers(-2 ** 31, 2 ** 31))
+            rows.append(r)
+    return [rows[i] for i in rng.permutation(len(rows))]
+
+
+def test_final_combine_of_partial_rows(eng):
+    """count(*), count(x), sum(int4) with NULL partials, int/date/float8 min and max, float8 sum and avg: the device FINAL
+    equals the oracle's combine functions (int8pl, float8pl, float8_combine, int4/int8/date/float8 larger/smaller)"""
+    from greengage_b200.engine import agg_final
+    fin = _final_agg()
+    rows = _partial_rows([-7, -1, 0, 3, 2 ** 31 - 1, -2 ** 31, None], 5, seed=1)
+    rows += _partial_rows([11], 3, seed=2, null_rate=1.0)             # every partial state NULL: sums and extremes NULL
+    got, want = agg_final(eng, fin, rows), po.agg_final(fin, rows)
+    assert len(got) == len(want) == 8
+    assert_aggrows_match(got, want, fin, float_exact=True)
+
+
+def test_final_combine_of_infinite_and_overflowing_float8_sums(eng):
+    """float8pl at the FINAL stage: an infinite partial sum makes an infinite sum; finite partials whose sum overflows are
+    an ERROR ("value out of range: overflow"), as in the oracle"""
+    from greengage_b200.engine import agg_final
+    fin = _final_agg([capi.AGG_SUM_FLOAT8, capi.AGG_AVG_FLOAT8])
+
+    def rows(parts):
+        out = []
+        for k, s in parts:
+            r = capi.gg_aggrow()
+            r.key[0] = k
+            r.agg[0].f[0] = s
+            r.agg[1].f[0], r.agg[1].f[1], r.agg[1].f[2] = 1.0, s, 0.0
+            out.append(r)
+        return out
+
+    inf = rows([(1, float("inf")), (1, 1.0), (2, 2.0), (2, 3.0), (3, float("-inf")), (3, -1e308)])
+    got, want = agg_final(eng, fin, inf), po.agg_final(fin, inf)
+    assert_aggrows_match(got, want, fin, float_exact=True)
+    assert sorted(r.agg[0].f[0] for r in got) == [float("-inf"), 5.0, float("inf")]
+    over = rows([(1, 1.7e308), (1, 1.7e308), (2, 1.0)])
+    with pytest.raises(po.OracleError):
+        po.agg_final(fin, over)
+    with pytest.raises(capi.GGError) as e:
+        agg_final(eng, fin, over)
+    assert e.value.code == -2
+
+
+def test_final_plain_aggregate_over_no_rows(eng):
+    """a plain FINAL Agg over no partial rows returns its one row: counts 0, everything else NULL"""
+    from greengage_b200.engine import agg_final
+    fin = _final_agg(keys=())
+    got, want = agg_final(eng, fin, []), po.agg_final(fin, [])
+    assert len(got) == len(want) == 1 and got[0].agg[0].i == got[0].agg[1].i == 0 and got[0].agg[2].isnull
+    assert_aggrows_match(got, want, fin, float_exact=True)
+
+
+def test_final_combine_of_more_groups_than_a_pipeline_holds(eng):
+    """1500 groups from 3 partial rows each: above the pooled group-set size (256) and a pipeline's merge capacity (1024)"""
+    from greengage_b200.engine import agg_final
+    fin = _final_agg()
+    rows = _partial_rows(range(-700, 800), 3, seed=3)
+    got, want = agg_final(eng, fin, rows), po.agg_final(fin, rows)
+    assert len(got) == len(want) == 1500
+    assert_aggrows_match(got, want, fin, float_exact=True)
+
+
+def test_device_final_over_a_pipeline_with_hundreds_of_groups(eng):
+    """Groups.of(pipeline).final(): a FINAL Agg directly over a PARTIAL pipeline's records (no Motion between them) with 600
+    groups, more than a pooled group set (256) holds.  The key is clustered and every run covers one page, so no block sees
+    more groups than its table holds and the pipeline keeps its groups as merged records."""
+    from greengage_b200.engine import Groups, Relation, ScanAgg
+    desc = make_desc([(capi.INT4OID, 4, "i", 1, 1), (capi.FLOAT8OID, 8, "d", 1, 1), (capi.INT4OID, 4, "i", 1, 0)])
+    rng = np.random.default_rng(5)
+    data, nulls = [], []
+    for k in range(600):
+        for _ in range(50):
+            data.append([k * 7 - 2000, float(rng.integers(-400, 400)) / 4, int(rng.integers(-1000, 1000))])
+            nulls.append([0, 0, int(rng.random() < 0.2)])
+    pages = po.build_pages(desc, data, nulls)
+    p = ExprPool()
+    k, x, i = p.var(1, capi.INT4OID), p.var(2, capi.FLOAT8OID), p.var(3, capi.INT4OID)
+    scan = capi.make_scan(desc, -1)
+    pagg = capi.make_agg(capi.AGGSTAGE_PARTIAL, [k], [(capi.AGG_COUNT_STAR, -1), (capi.AGG_COUNT_ANY, i), (capi.AGG_SUM_INT4, i),
+                                                     (capi.AGG_MIN_INT4, i), (capi.AGG_MAX_FLOAT8, x), (capi.AGG_SUM_FLOAT8, x),
+                                                     (capi.AGG_AVG_FLOAT8, x)])
+    fin = capi.gg_agg()
+    C.memmove(C.byref(fin), C.byref(pagg), C.sizeof(capi.gg_agg))
+    fin.aggstage, fin.grpCol[0] = capi.AGGSTAGE_FINAL, capi.INT4OID
+    rel = Relation(eng, host_pages=pages)
+    sa = ScanAgg(eng, scan, pagg, p.pool)
+    try:
+        for b in range(rel.nblocks):
+            sa.run(rel, b, 1)
+        part, sc, _ = sa.fetch()
+        assert sa.variant() % 16 != 5 and sc == len(data) and len(part) == 600
+        want, _, _, want_x = po.seqscan_agg(scan, pagg, p.pool, pages, exact=True)
+        assert_aggrows_match(part, want, pagg, exact=want_x)
+        g = Groups.of(sa)
+        f = g.final()
+        try:
+            got, _, _ = f.fetch()
+        finally:
+            f.free()
+            g.free()
+        assert len(got) == 600
+        assert_aggrows_match(got, po.agg_final(fin, part), fin, float_exact=True)
+    finally:
+        sa.free()
+        rel.free()
+
+
 def test_large_relation_properties(eng):
     """2 x 10^7 rows: counts are exact, halves add up to the whole, rows scanned == rows generated."""
     pages, nb, nr = tpch.synth_generate(tpch.synth_spec(capi.TAB_LINEITEM_NARROW, 20_000_000, seed=42))
