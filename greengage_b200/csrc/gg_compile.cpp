@@ -975,13 +975,23 @@ static bool check_desc(Ctx &c, const gg_tupdesc *d)
 	return true;
 }
 
-static int join_keytype(int32_t t)
+/* The key type (ggp_program::keytype) of a join key pair, or 0 when the reference cannot hash-join the pair: both sides must
+ * be in one hash opfamily (pg_amop.h:557-565 and the hash opclasses of pg_opclass.h).  Only integer_ops is cross-type here
+ * (int4 = int8; both load sign-extended to 64 bits and hashint8 agrees with hashint4 on int4 values).  Date, timestamp, bool,
+ * float8 and bpchar each hash only against their own type — date = timestamp compares days with microseconds, bpchar strips
+ * blanks where text does not — and varchar uses text's operators (text_ops). */
+static int join_keytype(int32_t outer, int32_t inner)
 {
-	switch (t)
+	const bool oint = outer == GG_INT4OID || outer == GG_INT8OID, iint = inner == GG_INT4OID || inner == GG_INT8OID;
+	const bool otext = outer == GG_VARCHAROID || outer == GG_TEXTOID, itext = inner == GG_VARCHAROID || inner == GG_TEXTOID;
+	if (oint && iint) return 1;
+	if (otext && itext) return 3;
+	if (outer != inner) return 0;
+	switch (outer)
 	{
-		case GG_INT4OID: case GG_INT8OID: case GG_DATEOID: case GG_TIMESTAMPOID: case GG_BOOLOID: return 1;
+		case GG_DATEOID: case GG_TIMESTAMPOID: case GG_BOOLOID: return 1;
 		case GG_FLOAT8OID: return 2;
-		case GG_BPCHAROID: case GG_VARCHAROID: case GG_TEXTOID: return 3;
+		case GG_BPCHAROID: return 3;
 	}
 	return 0;
 }
@@ -1037,9 +1047,8 @@ int ggp_compile_join(const gg_scan *outer, const gg_scan *inner, const gg_hashjo
 	gen_qual(c, outer->qual);
 	for (int k = 0; k < hj->nkeys && !c.failed; k++)
 	{
-		int kt = join_keytype(pool->nodes[hj->outerkey[k]].rettype);
-		int kti = join_keytype(pool->nodes[hj->innerkey[k]].rettype);
-		if (!kt || kt != kti) { fail(c, "join key %d: types %d / %d not hash-joinable on the GPU path", k, pool->nodes[hj->outerkey[k]].rettype, pool->nodes[hj->innerkey[k]].rettype); break; }
+		const int kt = join_keytype(pool->nodes[hj->outerkey[k]].rettype, pool->nodes[hj->innerkey[k]].rettype);
+		if (!kt) { fail(c, "join key %d: types %d / %d share no hash opfamily", k, pool->nodes[hj->outerkey[k]].rettype, pool->nodes[hj->innerkey[k]].rettype); break; }
 		jp->keytype[k] = (uint8_t) kt;
 		ggp_op *o = gen_value(c, hj->outerkey[k]);
 		if (c.failed) break;
@@ -1136,16 +1145,8 @@ int ggp_compile_motion(const gg_scan *scan, const gg_exprpool *pool, const int32
 	gen_qual(c, scan->qual);
 	for (int k = 0; k < nkeys && !c.failed; k++)
 	{
-		switch (pool->nodes[hashkeys[k]].rettype)
-		{
-			case GG_INT4OID: case GG_DATEOID: hashtype[k] = GGP_HT_INT4; break;
-			case GG_INT8OID: case GG_TIMESTAMPOID: hashtype[k] = GGP_HT_INT8; break;
-			case GG_FLOAT8OID: hashtype[k] = GGP_HT_FLOAT8; break;
-			case GG_BPCHAROID: case GG_VARCHAROID: case GG_TEXTOID: hashtype[k] = GGP_HT_STR; break;
-			case GG_BOOLOID: hashtype[k] = GGP_HT_BOOL; break;
-			default: fail(c, "hash key %d: type %d has no GPU hash function", k, pool->nodes[hashkeys[k]].rettype); break;
-		}
-		if (c.failed) break;
+		hashtype[k] = (uint8_t) ggp_hashtype_of(pool->nodes[hashkeys[k]].rettype);
+		if (!hashtype[k]) { fail(c, "hash key %d: type %d has no GPU hash function", k, pool->nodes[hashkeys[k]].rettype); break; }
 		ggp_op *o = gen_value(c, hashkeys[k]);
 		if (c.failed) break;
 		if (o->flags & GGP_F_KEY) { emit(c, GGP_NOP); o = &prog->code[prog->ncode - 1]; }

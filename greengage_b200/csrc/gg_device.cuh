@@ -127,6 +127,19 @@ __device__ __forceinline__ uint32_t hashfloat8(uint64_t bits)
 	if (d == 0.0) return 0;
 	return hash_any_le8(bits, 8);
 }
+/* the hash of one non-NULL Motion / distribution key value (cdbhash.c:215-287: the type's default hash opclass function), by
+ * ggp_hashtype.  A string arrives packed LSB-first (bpchar already blank-stripped): its length is where its first zero byte is.
+ * The one copy of this dispatch: the sending Motion (PartSink), the group-record Motion (route_group) and the emulator use it. */
+__device__ __forceinline__ uint32_t key_hash(int t, uint64_t v)
+{
+	if (t == GGP_HT_INT4) return hash_uint32((uint32_t) v);
+	if (t == GGP_HT_INT8) return hashint8((int64_t) v);
+	if (t == GGP_HT_FLOAT8) return hashfloat8(v);
+	if (t == GGP_HT_BOOL) return hash_uint32((uint32_t) (int32_t) (int8_t) v);      /* hashchar */
+	int len = 0;
+	while (len < 8 && ((v >> (8 * len)) & 0xff)) len++;
+	return hash_any_le8(v, len);
+}
 /* cdbhash.c:197-219: rotate left 1, xor the column hash unless NULL */
 __device__ __forceinline__ uint32_t cdbhash_add(uint32_t h, uint32_t hk, bool isnull)
 {
@@ -490,7 +503,7 @@ static __device__ __noinline__ uint32_t f8_check_slow(int kind /* 0 add/sub, 1 m
 	return e;
 }
 
-/* normalise a grouping key so that bitwise equality == SQL equality for grouping */
+/* normalise a key so that bitwise equality == SQL equality (join keys: the hash table compares bits) */
 __device__ __forceinline__ uint64_t normalize_key(uint64_t v, int keytype)
 {
 	if (keytype == 2)
@@ -501,6 +514,23 @@ __device__ __forceinline__ uint64_t normalize_key(uint64_t v, int keytype)
 	}
 	return v;
 }
+/* A grouping key as its group stores it.  The group's key is the value of the row that created the group
+ * (lookup_agg_hash_entry, execHHashagg.c:456 copies the first tuple's), so a float8 zero keeps its sign; every NaN becomes one
+ * encoding, because records are routed and merged by their key bits.  Grouping keys are compared with key_same and hashed
+ * (HashAggregate) as normalize_key gives them. */
+__device__ __forceinline__ uint64_t group_key(uint64_t v, int keytype)
+{
+	if (keytype == 2 && __longlong_as_double((long long) v) != __longlong_as_double((long long) v)) return 0x7ff8000000000000ull;
+	return v;
+}
+/* two group_key values are one group: equal bits, or (f8: a float8 key) zeros of either sign */
+__device__ __forceinline__ bool key_same(uint64_t a, uint64_t b, bool f8)
+{
+	return a == b || (f8 && ((a | b) << 1) == 0);
+}
+/* of 2-bit key types (key c at bits 2c): bit 2c set where key c is float8.  A constant with no float8 key folds to 0, so a
+ * plan-specialised kernel without one compares its keys as plain bits */
+__device__ __forceinline__ uint32_t f8_keys(uint32_t keytypes) { return (keytypes >> 1) & ~keytypes & 0x55u; }
 
 /* Everything a running program needs to reach its operands */
 struct EvalCtx {

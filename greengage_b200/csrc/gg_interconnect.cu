@@ -178,22 +178,7 @@ __device__ __forceinline__ int route_group(const ggp_grec &r, int nhash, const i
 		const int c = hashcol[k];
 		const bool isnull = (r.keynull >> c) & 1;
 		const uint64_t v = r.key[c];
-		uint32_t hk = 0;
-		if (!isnull)
-		{
-			const int t = hashtype[k];
-			if (t == GGP_HT_INT4) hk = hash_uint32((uint32_t) v);
-			else if (t == GGP_HT_INT8) hk = hashint8((int64_t) v);
-			else if (t == GGP_HT_FLOAT8) hk = hashfloat8(v);
-			else if (t == GGP_HT_BOOL) hk = hash_uint32((uint32_t) (int32_t) (int8_t) v);
-			else
-			{
-				int len = 0;
-				while (len < 8 && ((v >> (8 * len)) & 0xff)) len++;
-				hk = hash_any_le8(v, len);
-			}
-		}
-		h = cdbhash_add(h, hk, isnull);
+		h = cdbhash_add(h, isnull ? 0 : key_hash(hashtype[k], v), isnull);
 	}
 	return jump_consistent_hash((uint64_t) h, nsegs);
 }
@@ -566,15 +551,8 @@ int gg_ic_motion_groups(gg_interconnect *ic, int motion_type, int root, int nhas
 		if (hashcol[k] < 0 || (in && hashcol[k] >= in->nkeys))
 		{ gg_set_error("Motion hash column %d is not a grouping column of the rows below", hashcol[k]); return GG_ERR_UNSUPPORTED; }
 		spec.hashcol[k] = hashcol[k];
-		switch (hashtypid[k])
-		{
-			case GG_INT4OID: case GG_DATEOID: spec.hashtype[k] = GGP_HT_INT4; break;
-			case GG_INT8OID: case GG_TIMESTAMPOID: spec.hashtype[k] = GGP_HT_INT8; break;
-			case GG_FLOAT8OID: spec.hashtype[k] = GGP_HT_FLOAT8; break;
-			case GG_BPCHAROID: case GG_VARCHAROID: case GG_TEXTOID: spec.hashtype[k] = GGP_HT_STR; break;
-			case GG_BOOLOID: spec.hashtype[k] = GGP_HT_BOOL; break;
-			default: gg_set_error("hash column type %d has no device hash function", hashtypid[k]); return GG_ERR_UNSUPPORTED;
-		}
+		spec.hashtype[k] = ggp_hashtype_of(hashtypid[k]);
+		if (!spec.hashtype[k]) { gg_set_error("hash column type %d has no device hash function", hashtypid[k]); return GG_ERR_UNSUPPORTED; }
 	}
 	gg_groups *g = gg_groups_alloc(e, in, ic->nsegs * GG_IC_GROUP_CAP, /*sparse*/ true);
 	if (!g) return GG_ERR_NOMEM;

@@ -222,6 +222,20 @@ static inline int ggp_acckind_of(int32_t aggfnoid)
 		default: return -1;
 	}
 }
+/* the ggp_hashtype of a key type (cdb_hashproc_in_opfamily, cdbhash.c:135-165: date hashes as int4, timestamp as int8, bool as
+ * hashchar, bpchar blank-stripped); 0 for a type the device cannot hash */
+static inline int ggp_hashtype_of(int32_t typid)
+{
+	switch (typid)
+	{
+		case GG_INT4OID: case GG_DATEOID: return GGP_HT_INT4;
+		case GG_INT8OID: case GG_TIMESTAMPOID: return GGP_HT_INT8;
+		case GG_FLOAT8OID: return GGP_HT_FLOAT8;
+		case GG_BPCHAROID: case GG_VARCHAROID: case GG_TEXTOID: return GGP_HT_STR;
+		case GG_BOOLOID: return GGP_HT_BOOL;
+		default: return 0;
+	}
+}
 int ggp_compile_scanagg(const gg_scan *scan, const gg_agg *agg, const gg_exprpool *pool,
                         ggp_program *prog, ggp_aggmap *aggmap, char *err, int errlen);
 int ggp_disasm(const ggp_program *p, char *buf, int cap);

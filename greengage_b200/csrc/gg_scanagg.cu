@@ -85,13 +85,19 @@ __global__ void gg_hashagg_emit_kernel(HashAggTable ha, ggp_grec *out, unsigned 
 	}
 }
 
-/* ---- merge kernel: fold group records with equal keys, in record order (deterministic) ----
+/* the key types of a program or group set, 2 bits per key as the kernels take them */
+static inline uint32_t keytypes_of(const uint8_t *kt)
+{
+	return (uint32_t) kt[0] | ((uint32_t) kt[1] << 2) | ((uint32_t) kt[2] << 4) | ((uint32_t) kt[3] << 6);
+}
+
+/* ---- merge kernel: fold group records with equal keys (key_same), in record order (deterministic) ----
  * One block.  A: ordered compaction of the valid records.  B: every valid record finds (or, under a
  * lock, creates) its merged group.  C: thread (group, column) folds that group's records in record
  * order.  This is also the combine step of a FINAL-stage Agg (float8pl / float8_combine / int8pl,
  * nodeAgg.c:2123-2148) when the records come from other segments. */
 __global__ void __launch_bounds__(1024, 1)
-gg_merge_recs_kernel(const ggp_grec *recs, int nrecs, int nkeys, int nacc, ggp_acckinds kinds,
+gg_merge_recs_kernel(const ggp_grec *recs, int nrecs, int nkeys, uint32_t keytypes, int nacc, ggp_acckinds kinds,
                      ggp_grec *out, int outcap, int *nout, int *vidx /* [nrecs] */, int *vmap /* [nrecs] */,
                      uint32_t *errflags, int prefix_sets /* 1: the valid records of a set are a prefix of it */)
 {
@@ -135,7 +141,7 @@ gg_merge_recs_kernel(const ggp_grec *recs, int nrecs, int nkeys, int nacc, ggp_a
 			for (int m = 0; m < n && f < 0; m++)
 			{
 				bool eq = out[m].keynull == x->keynull;
-				for (int c = 0; eq && c < nkeys; c++) eq = out[m].key[c] == x->key[c];
+				for (int c = 0; eq && c < nkeys; c++) eq = key_same(out[m].key[c], x->key[c], (f8_keys(keytypes) >> (2 * c)) & 1);
 				if (eq) f = m;
 			}
 			need = f < 0;
@@ -152,7 +158,7 @@ gg_merge_recs_kernel(const ggp_grec *recs, int nrecs, int nkeys, int nacc, ggp_a
 				for (int m = 0; m < n && f < 0; m++)
 				{
 					bool eq = ((volatile ggp_grec *) out)[m].keynull == x->keynull;
-					for (int c = 0; eq && c < nkeys; c++) eq = ((volatile ggp_grec *) out)[m].key[c] == x->key[c];
+					for (int c = 0; eq && c < nkeys; c++) eq = key_same(((volatile ggp_grec *) out)[m].key[c], x->key[c], (f8_keys(keytypes) >> (2 * c)) & 1);
 					if (eq) f = m;
 				}
 				if (f < 0)
@@ -180,7 +186,7 @@ gg_merge_recs_kernel(const ggp_grec *recs, int nrecs, int nkeys, int nacc, ggp_a
 				for (int m = 0; m < n && f < 0; m++)
 				{
 					bool eq = ((volatile ggp_grec *) out)[m].keynull == x->keynull;
-					for (int c = 0; eq && c < nkeys; c++) eq = ((volatile ggp_grec *) out)[m].key[c] == x->key[c];
+					for (int c = 0; eq && c < nkeys; c++) eq = key_same(((volatile ggp_grec *) out)[m].key[c], x->key[c], (f8_keys(keytypes) >> (2 * c)) & 1);
 					if (eq) f = m;
 				}
 				need = f < 0;
@@ -442,7 +448,7 @@ int scanagg_launch(gg_scanagg *p, const uint8_t *dev_pages, uint64_t nblocks, cu
 	/* fold the block records (and the previously merged groups) */
 	ggp_acckinds kinds;
 	memcpy(kinds.k, p->prog.acckind, sizeof kinds.k);
-	gg_merge_recs_kernel<<<1, 1024, 0, st>>>(p->recs, p->nrecs_total, p->prog.nkeys, p->prog.nacc, kinds,
+	gg_merge_recs_kernel<<<1, 1024, 0, st>>>(p->recs, p->nrecs_total, p->prog.nkeys, keytypes_of(p->prog.keytype), p->prog.nacc, kinds,
 	                                        p->merged, GG_MERGE_CAP, p->d_nout, p->vidx, p->vmap, p->d_err, 1);
 	GG_CUDA(cudaGetLastError());
 	e->launches++;
@@ -1053,8 +1059,9 @@ int gg_agg_final(gg_engine *e, const gg_agg *agg, const gg_aggrow *in, int nin,
 				uint64_t k = (uint64_t) in[r].key[c];
 				if (like.keytype[c] == 2)
 				{
+					/* group_key: a zero keeps its sign, the merge compares ±0 alike; NaNs are one key */
 					double d; memcpy(&d, &k, 8);
-					if (d == 0.0) k = 0; else if (d != d) k = 0x7ff8000000000000ull;
+					if (d != d) k = 0x7ff8000000000000ull;
 				}
 				else if (agg->grpCol[c] == GG_INT4OID || agg->grpCol[c] == GG_DATEOID)
 					k = (uint64_t) (int64_t) (int32_t) k;
@@ -1191,7 +1198,7 @@ int gg_groups_final(gg_engine *e, gg_groups *in, gg_groups **out)
 	if (ce == cudaSuccess) ce = cudaMemsetAsync(g->recs, 0, sizeof(ggp_grec) * (size_t) cap, st);
 	if (ce == cudaSuccess)
 	{
-		gg_merge_recs_kernel<<<1, 1024, 0, st>>>(in->recs, cap, in->nkeys, in->nacc, kinds, g->recs, cap, g->d_n,
+		gg_merge_recs_kernel<<<1, 1024, 0, st>>>(in->recs, cap, in->nkeys, keytypes_of(in->keytype), in->nacc, kinds, g->recs, cap, g->d_n,
 		                                        g->scratch, g->scratch + g->alloc_cap, &g->d_status->err, in->sparse ? 0 : 1);
 		ce = cudaGetLastError();
 		e->launches++;

@@ -238,17 +238,17 @@ struct BlockTable {                       /* per-block group table in shared mem
 	int lock;
 };
 
-__device__ __forceinline__ bool key_eq(const BlockTable *T, int i, const uint64_t *k, uint32_t knull, int nkeys)
+__device__ __forceinline__ bool key_eq(const BlockTable *T, int i, const uint64_t *k, uint32_t knull, int nkeys, uint32_t keytypes)
 {
 	if (T->keynull[i] != knull) return false;
 	for (int c = 0; c < nkeys; c++)
-		if (T->key[i][c] != k[c]) return false;
+		if (!key_same(T->key[i][c], k[c], (f8_keys(keytypes) >> (2 * c)) & 1)) return false;
 	return true;
 }
 
 /* find the group of each lane's key, inserting new groups under a block-level lock
  * (lookup_agg_hash_entry, execHHashagg.c:456: NULL keys compare equal to each other) */
-__device__ __forceinline__ int find_or_insert(BlockTable *T, const uint64_t *k, uint32_t knull, int nkeys,
+__device__ __forceinline__ int find_or_insert(BlockTable *T, const uint64_t *k, uint32_t knull, int nkeys, uint32_t keytypes,
                                               int gcap, bool want, int lane, uint32_t &err)
 {
 	int gid = -1;
@@ -257,7 +257,7 @@ __device__ __forceinline__ int find_or_insert(BlockTable *T, const uint64_t *k, 
 	{
 		int n = T->n;
 		for (int i = 0; i < n; i++)
-			if (key_eq(T, i, k, knull, nkeys)) { gid = i; break; }
+			if (key_eq(T, i, k, knull, nkeys, keytypes)) { gid = i; break; }
 		need = gid < 0;
 	}
 	unsigned m = __ballot_sync(GG_FULL_MASK, need);
@@ -270,7 +270,7 @@ __device__ __forceinline__ int find_or_insert(BlockTable *T, const uint64_t *k, 
 			__threadfence_block();
 			int n = T->n, found = -1;
 			for (int i = 0; i < n; i++)
-				if (key_eq(T, i, k, knull, nkeys)) { found = i; break; }
+				if (key_eq(T, i, k, knull, nkeys, keytypes)) { found = i; break; }
 			if (found < 0)
 			{
 				if (n < gcap)
@@ -294,7 +294,7 @@ __device__ __forceinline__ int find_or_insert(BlockTable *T, const uint64_t *k, 
 		{
 			int n = T->n;
 			for (int i = 0; i < n; i++)
-				if (key_eq(T, i, k, knull, nkeys)) { gid = i; break; }
+				if (key_eq(T, i, k, knull, nkeys, keytypes)) { gid = i; break; }
 			need = gid < 0;
 		}
 		m = __ballot_sync(GG_FULL_MASK, need);
@@ -345,8 +345,12 @@ struct RowSink {
 	__device__ __forceinline__ void key(int kc, uint64_t v, bool isnull)
 	{
 		if (isnull) { knull |= 1u << kc; return; }
-		v = normalize_key(v, (int) ((keytypes >> (2 * kc)) & 3));
+		v = group_key(v, (int) ((keytypes >> (2 * kc)) & 3));
 		if (kc == 0) k0 = v; else if (kc == 1) k1 = v; else if (kc == 2) k2 = v; else k3 = v;
+	}
+	__device__ __forceinline__ bool same2(uint64_t a0, uint64_t a1) const
+	{
+		return key_same(k0, a0, f8_keys(keytypes) & 1) && key_same(k1, a1, (f8_keys(keytypes) >> 2) & 1);
 	}
 	/* the first groups of the block's table, cached in registers: with a handful of groups (Q1 has four) a row finds its group
 	 * by comparing against registers, and the shared-memory table (and its lock) is only visited for a key no lane of the warp
@@ -374,16 +378,23 @@ struct RowSink {
 			int g = -1;
 			if (knull == 0)
 			{
-				if (cn > 0 && k0 == c00 && k1 == c01) g = 0;
-				else if (cn > 1 && k0 == c10 && k1 == c11) g = 1;
-				else if (cn > 2 && k0 == c20 && k1 == c21) g = 2;
-				else if (cn > 3 && k0 == c30 && k1 == c31) g = 3;
+				if (f8_keys(keytypes) == 0)     /* no float8 key: equal bits are equal keys (a constant in a specialised kernel) */
+				{
+					if (cn > 0 && k0 == c00 && k1 == c01) g = 0;
+					else if (cn > 1 && k0 == c10 && k1 == c11) g = 1;
+					else if (cn > 2 && k0 == c20 && k1 == c21) g = 2;
+					else if (cn > 3 && k0 == c30 && k1 == c31) g = 3;
+				}
+				else if (cn > 0 && same2(c00, c01)) g = 0;
+				else if (cn > 1 && same2(c10, c11)) g = 1;
+				else if (cn > 2 && same2(c20, c21)) g = 2;
+				else if (cn > 3 && same2(c30, c31)) g = 3;
 			}
 			const bool need = live && g < 0;
 			if (__any_sync(GG_FULL_MASK, need))
 			{
 				uint64_t k[GG_MAX_KEYS] = { k0, k1, k2, k3 };
-				const int g2 = find_or_insert(T, k, knull, nkeys, gcap, need, lane, *err);
+				const int g2 = find_or_insert(T, k, knull, nkeys, keytypes, gcap, need, lane, *err);
 				if (need) g = g2;
 				cache_refresh();
 			}
@@ -392,7 +403,7 @@ struct RowSink {
 		else
 		{
 			uint64_t k[GG_MAX_KEYS] = { k0, k1, k2, k3 };
-			gid = find_or_insert(T, k, knull, nkeys, gcap, live, lane, *err);
+			gid = find_or_insert(T, k, knull, nkeys, keytypes, gcap, live, lane, *err);
 		}
 		if (live) npassed++;
 		if (MODE == MODE_PRIV && gid >= 0)
@@ -510,21 +521,7 @@ struct PartSink {
 	__device__ __forceinline__ bool filter(bool pass) { return pass; }
 	__device__ __forceinline__ void key(int kc, uint64_t v, bool isnull)
 	{
-		uint32_t hk = 0;
-		if (!isnull)
-		{
-			const int t = (int) ((mo.hashtypes >> (4 * kc)) & 15);
-			if (t == GGP_HT_INT4) hk = hash_uint32((uint32_t) v);
-			else if (t == GGP_HT_INT8) hk = hashint8((int64_t) v);
-			else if (t == GGP_HT_FLOAT8) hk = hashfloat8(v);
-			else if (t == GGP_HT_BOOL) hk = hash_uint32((uint32_t) (int32_t) (int8_t) v);
-			else
-			{
-				int len = 0;
-				while (len < 8 && ((v >> (8 * len)) & 0xff)) len++;
-				hk = hash_any_le8(v, len);
-			}
-		}
+		const uint32_t hk = isnull ? 0 : key_hash((int) ((mo.hashtypes >> (4 * kc)) & 15), v);
 		h = cdbhash_add(h, hk, isnull);
 	}
 	__device__ __forceinline__ bool group(bool live)
@@ -596,7 +593,7 @@ struct HashSink {
 	__device__ __forceinline__ void key(int kc, uint64_t v, bool isnull)
 	{
 		if (isnull) { knull |= 1u << kc; return; }
-		v = normalize_key(v, (int) ((keytypes >> (2 * kc)) & 3));
+		v = group_key(v, (int) ((keytypes >> (2 * kc)) & 3));
 		if (kc == 0) k0 = v; else if (kc == 1) k1 = v; else if (kc == 2) k2 = v; else k3 = v;
 	}
 	__device__ __forceinline__ bool group(bool live)
@@ -604,7 +601,10 @@ struct HashSink {
 		if (suppress) live = false;
 		if (!live) return false;
 		npassed++;
-		uint64_t h = join_hash(k0 ^ (k2 * 0xD6E8FEB86659FD93ull), k1 ^ (k3 * 0xA0761D6478BD642Full) ^ ((uint64_t) knull << 56));
+		/* hashed normalised (both zeros alike), compared with key_same; the entry keeps the inserting row's key */
+		const int t0 = (int) (keytypes & 3), t1 = (int) ((keytypes >> 2) & 3), t2 = (int) ((keytypes >> 4) & 3), t3 = (int) ((keytypes >> 6) & 3);
+		uint64_t h = join_hash(normalize_key(k0, t0) ^ (normalize_key(k2, t2) * 0xD6E8FEB86659FD93ull),
+		                       normalize_key(k1, t1) ^ (normalize_key(k3, t3) * 0xA0761D6478BD642Full) ^ ((uint64_t) knull << 56));
 		const unsigned long long ready = 0x8000000000000000ull | ((unsigned long long) knull << 32) | (uint32_t) h;
 		uint64_t slot = (h >> 32) & (ha.cap - 1);
 		/* a probe sequence this long means the table is overloaded: report it full so that the host rebuilds it larger */
@@ -633,7 +633,8 @@ struct HashSink {
 			if (cur == ready)
 			{
 				const volatile unsigned long long *kp = ep + 1;
-				if ((ha.nkeys < 1 || kp[0] == k0) && (ha.nkeys < 2 || kp[1] == k1) && (ha.nkeys < 3 || kp[2] == k2) && (ha.nkeys < 4 || kp[3] == k3))
+				if ((ha.nkeys < 1 || key_same(kp[0], k0, t0 == 2)) && (ha.nkeys < 2 || key_same(kp[1], k1, t1 == 2)) &&
+				    (ha.nkeys < 3 || key_same(kp[2], k2, t2 == 2)) && (ha.nkeys < 4 || key_same(kp[3], k3, t3 == 2)))
 				{ e = (long long) slot; break; }
 			}
 			slot = (slot + 1) & (ha.cap - 1);
@@ -1283,7 +1284,8 @@ __device__ __forceinline__ void scanagg_body(const ggp_program &P, const ScanAgg
 					sink.keytypes = jt.keytypes;
 					PL::template run_range<NULLABLE>(X, M1, 0, jt.probe_pc, err, sink);
 					sink.keytypes = gkt;
-					const uint64_t jk0 = sink.k0, jk1 = sink.k1;
+					/* the sink keeps a zero's sign (group_key); the hash table holds join keys normalised */
+					const uint64_t jk0 = normalize_key(sink.k0, (int) (jt.keytypes & 3)), jk1 = normalize_key(sink.k1, (int) ((jt.keytypes >> 2) & 3));
 					const bool jknull = sink.knull != 0;
 					bool pending = M1.live && (fill_outer || !jknull);     /* a NULL key matches nothing (nodeHash.c:1070) */
 					if (lasj && jknull && !jt.inner_empty) pending = false;     /* NULL NOT IN (non-empty set): dropped (nodeHashjoin.c:361) */

@@ -107,8 +107,15 @@ keys_match(const gg_exprpool *pool, const gg_hashjoin *hj, or_row *outer, or_row
 			else
 				*match = (a.len == b.len && memcmp(a.ptr, b.ptr, (size_t) a.len) == 0);
 		}
-		else if (typ == GG_INT4OID || typ == GG_DATEOID)
-			*match = (int32_t) a.v == (int32_t) b.v;
+		else if (typ == GG_INT4OID || typ == GG_DATEOID || typ == GG_INT8OID)
+		{
+			/* int4eq / int48eq / int84eq / int8eq (integer_ops): each side widened from its own type, never truncated */
+			int32_t ityp = pool->nodes[hj->innerkey[i]].rettype;
+			int64_t x = (typ == GG_INT8OID) ? a.v : (int64_t) (int32_t) a.v;
+			int64_t y = (ityp == GG_INT8OID || ityp == GG_TIMESTAMPOID) ? b.v : (int64_t) (int32_t) b.v;
+
+			*match = x == y;
+		}
 		else if (typ == GG_FLOAT8OID)
 		{
 			double x, y;

@@ -42,13 +42,13 @@ struct HostSink {
 	void key(int kc, uint64_t v, bool isnull)
 	{
 		if (isnull) { knull |= 1u << kc; return; }
-		k[kc] = normalize_key(v, P->keytype[kc]);
+		k[kc] = group_key(v, P->keytype[kc]);
 	}
 	bool group(bool live)
 	{
 		if (!live) { cur = nullptr; return false; }
 		std::array<uint64_t, GG_MAX_KEYS + 1> id;
-		for (int i = 0; i < GG_MAX_KEYS; i++) id[i] = (i < P->nkeys && !((knull >> i) & 1)) ? k[i] : 0;
+		for (int i = 0; i < GG_MAX_KEYS; i++) id[i] = (i < P->nkeys && !((knull >> i) & 1)) ? normalize_key(k[i], P->keytype[i]) : 0;
 		id[GG_MAX_KEYS] = knull;
 		auto it = groups.find(id);
 		if (it == groups.end())
@@ -57,7 +57,7 @@ struct HostSink {
 			memset(&g, 0, sizeof g);
 			for (int j = 0; j < P->nacc; j++)                  /* float8 sums start from -0, as the kernels' accumulators do */
 				if (P->acckind[j] == GGP_ACC_F8SUM) g.sum[j] = -0.0;
-			for (int i = 0; i < GG_MAX_KEYS; i++) g.key[i] = id[i];
+			for (int i = 0; i < GG_MAX_KEYS; i++) g.key[i] = (i < P->nkeys && !((knull >> i) & 1)) ? k[i] : 0;     /* the first row's key */
 			g.keynull = knull;
 			it = groups.emplace(id, g).first;
 		}
@@ -197,19 +197,11 @@ extern "C" uint32_t emu_hashfloat8(uint64_t bits) { return hashfloat8(bits); }
 extern "C" uint32_t emu_hash_any_le8(uint64_t v, int len) { return hash_any_le8(v, len); }
 extern "C" int32_t emu_route(const int32_t *typids, const int64_t *vals, const int32_t *lens, const int32_t *isnull, int nkeys, int nsegs)
 {
+	/* the kernels' key_hash; a string's length is where its packed bytes end, so `lens` is not read */
+	(void) lens;
 	uint32_t h = 0;
 	for (int i = 0; i < nkeys; i++)
-	{
-		uint32_t hk = 0;
-		switch (typids[i])
-		{
-			case GG_INT4OID: case GG_DATEOID: hk = hash_uint32((uint32_t) (int32_t) vals[i]); break;
-			case GG_INT8OID: case GG_TIMESTAMPOID: hk = hashint8(vals[i]); break;
-			case GG_FLOAT8OID: hk = hashfloat8((uint64_t) vals[i]); break;
-			default: hk = hash_any_le8((uint64_t) vals[i], lens[i]); break;       /* packed, blank-stripped strings */
-		}
-		h = cdbhash_add(h, hk, isnull[i] != 0);
-	}
+		h = cdbhash_add(h, isnull[i] ? 0 : key_hash(ggp_hashtype_of(typids[i]), (uint64_t) vals[i]), isnull[i] != 0);
 	return jump_consistent_hash((uint64_t) h, nsegs);
 }
 

@@ -145,6 +145,40 @@ def test_join_shapes_outside_the_subset_are_refused():
     assert e.value.code == -6 and "join key" in str(e.value)
 
 
+KEY_TYPES = {"int4": (capi.INT4OID, 4, "i", 1), "int8": (capi.INT8OID, 8, "d", 1), "date": (capi.DATEOID, 4, "i", 1),
+             "timestamp": (capi.TIMESTAMPOID, 8, "d", 1), "bool": (capi.BOOLOID, 1, "c", 1), "float8": (capi.FLOAT8OID, 8, "d", 1),
+             "bpchar": (capi.BPCHAROID, -1, "i", 0), "varchar": (capi.VARCHAROID, -1, "i", 0), "text": (capi.TEXTOID, -1, "i", 0)}
+# the pairs the reference can hash-join: one hash opfamily per pair (pg_amop.h:557-565).  integer_ops is the only cross-type
+# family among these types; varchar has no operators of its own and uses text_ops.
+HASH_JOINABLE = {frozenset(p) for p in (("int4",), ("int8",), ("int4", "int8"), ("date",), ("timestamp",), ("bool",), ("float8",),
+                                         ("bpchar",), ("varchar",), ("text",), ("varchar", "text"))}
+
+
+@pytest.mark.parametrize("nkeys", [1, 2])
+def test_join_key_pairs_follow_the_reference_hash_opfamilies(nkeys):
+    """Every (outer, inner) pair of device key types: compiled when the reference can hash-join it, GG_ERR_UNSUPPORTED with a
+    message naming the join key otherwise — date = timestamp, bpchar = text, int4 = date, int4 = bool, float8 = int8 and the
+    like must never compile into a bitwise comparison of unlike encodings.  With two keys the pair is the second key."""
+    names = list(KEY_TYPES)
+    desc = make_desc([KEY_TYPES[n] for n in names])
+    for i, a in enumerate(names):
+        for j, b in enumerate(names):
+            p = ExprPool()
+            ok, ik = [p.var(i + 1, KEY_TYPES[a][0], 0)], [p.var(j + 1, KEY_TYPES[b][0], 1)]
+            if nkeys == 2:
+                ok, ik = [p.var(1, capi.INT4OID, 0)] + ok, [p.var(1, capi.INT4OID, 1)] + ik
+            hj = capi.make_hashjoin(capi.JOIN_INNER, ok, ik)
+            agg = capi.make_agg(capi.AGGSTAGE_NORMAL, [], [(capi.AGG_COUNT_STAR, -1)])
+            args = (capi.make_scan(desc, -1), capi.make_scan(desc, -1), hj, agg, p.pool)
+            if frozenset((a, b)) in HASH_JOINABLE:
+                build, probe, text = disasm_join(*args)
+                assert "KEY%d PROBE" % (nkeys - 1) in text, (a, b, text)
+            else:
+                with pytest.raises(capi.GGError) as e:
+                    disasm_join(*args)
+                assert e.value.code == -6 and "join key %d" % (nkeys - 1) in str(e.value), (a, b, str(e.value))
+
+
 def test_datum_row_input_uses_constant_word_offsets():
     types = [capi.INT8OID, capi.FLOAT8OID, capi.BPCHAROID, capi.DATEOID]
     desc = capi.rows_tupdesc(types, notnull=[1, 1, 0, 1])

@@ -300,6 +300,48 @@ def test_device_hash_and_routing_functions_equal_the_references(emu):
     assert routed > 1000
 
 
+def test_device_routing_of_every_key_type_equals_the_oracle(emu):
+    """key_hash + cdbhash (the one hash dispatch the sending Motion and the group-record Motion run) against the oracle's
+    or_route_datums, which test_oracle_hash.py pins to the reference's cdbhash.o: every device key type — bool (hashchar),
+    date (hashint4), timestamp (hashint8), float8 ±0 / NaN / ±inf, bpchar stripped and varchar / text with their blanks —
+    alone and in keys of 2..4 columns with NULLs anywhere, over segment counts from 1 to 1024."""
+    import random
+    emu.emu_route.argtypes = [C.POINTER(C.c_int32), C.POINTER(C.c_int64), C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int, C.c_int]
+    rng = random.Random(17)
+    f8 = [0.0, -0.0, float("inf"), -float("inf"), float("nan"), 5e-324, 1.7976931348623157e308, 1.0, 1.0000000000000002, -2.5]
+    strs = [b"", b" ", b"A", b"A ", b"ABCDEFGH", b"ABCDEFG ", b"\x80\xff", b"ab", b"abc  "]
+
+    def value(t):
+        if t == capi.BOOLOID:
+            return rng.choice([0, 1]), 0
+        if t in (capi.INT4OID, capi.DATEOID):
+            return rng.choice([0, 1, -1, -2**31, 2**31 - 1, rng.randint(-2**31, 2**31 - 1)]), 0
+        if t in (capi.INT8OID, capi.TIMESTAMPOID):
+            return rng.choice([0, 2**32 + 1, -1, 2**32 - 1, -2**63, 2**63 - 1, rng.randint(-2**63, 2**63 - 1)]), 0
+        if t == capi.FLOAT8OID:
+            return f2b(rng.choice(f8)), 0
+        b = rng.choice(strs)
+        if t == capi.BPCHAROID:
+            b = b.rstrip(b" ")                                           # packed bpchar is blank-stripped
+        return int.from_bytes(b.ljust(8, b"\0"), "little", signed=True), len(b)
+
+    types = [capi.BOOLOID, capi.INT4OID, capi.DATEOID, capi.INT8OID, capi.TIMESTAMPOID, capi.FLOAT8OID, capi.BPCHAROID,
+             capi.VARCHAROID, capi.TEXTOID]
+    seen = set()
+    for it in range(6000):
+        n = 1 if it < 2000 else rng.randint(2, 4)
+        typ = [types[it % len(types)]] if n == 1 else [rng.choice(types) for _ in range(n)]
+        vl = [value(t) for t in typ]
+        nul = [0] * n if n == 1 and it % 10 else [int(rng.random() < 0.3) for _ in range(n)]
+        nsegs = rng.choice([1, 2, 3, 7, 8, 64, 1024])
+        t, v = (C.c_int32 * n)(*typ), (C.c_int64 * n)(*[x for x, _ in vl])
+        ln, nn = (C.c_int32 * n)(*[x for _, x in vl]), (C.c_int32 * n)(*nul)
+        want = po.lib().or_route_datums(t, v, ln, nn, n, nsegs)
+        assert emu.emu_route(t, v, ln, nn, n, nsegs) == want, (typ, vl, nul, nsegs)
+        seen.add(typ[0])
+    assert seen == set(types)
+
+
 def test_device_tuple_walk_equals_the_references_deform(emu):
     """walk_tuple (the GPU's slot_deform_tuple) over the 180 tuples the reference's heap_form_tuple built
     (tests/golden/heap_kat.json: NULL bitmaps, 1-byte and big-endian 4-byte varlena headers, alignment padding): every
