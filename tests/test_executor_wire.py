@@ -149,6 +149,28 @@ def test_rows_from_cpu_senders_arrive_at_the_motion_and_the_final_stage_combines
             assert abs(b2f(v[2 + col]) - w.agg[col].f[0]) <= 1e-9 * abs(w.agg[col].f[0])
 
 
+def test_finalised_rows_arrive_at_a_gather_above_a_final_agg(mock):
+    """Gather Motion <- Agg(FINAL) <- ...: finalised rows arrive as tuple chunks before the slice below has run, so the Motion
+    lays them out from the FINAL Agg's plan, whose grouping columns are key type OIDs (not expression roots)"""
+    eng = mock.mock_engine()
+    scan, one, pool1 = tpch.q1_plan(capi.TAB_LINEITEM_WIDE)
+    b = ex.PlanBuilder()
+    rel0 = MockRel(mock, shard(0))
+    x = ex.Executor(eng, pool1, [rel0], b.agg(b.seqscan(0, scan.desc, scan.qual), one))
+    out = (C.c_uint8 * 65536)()
+    got = mock.GgExecSendTupleChunks(x.state, 8124, out, len(out), None)
+    assert got > 0, mock.GgExecLastError()
+    sent = x.rows()
+    x.end()
+    assert len(sent) == 4
+    scan, part, pool = tpch.q1_plan(capi.TAB_LINEITEM_WIDE, capi.AGGSTAGE_PARTIAL)
+    below = b.agg(b.motion(b.agg(b.seqscan(0, scan.desc, scan.qual), part), ex.MOTION_GATHER, [], 1), tpch.q1_final_agg(part))
+    x = ex.Executor(eng, pool, [rel0], b.motion(below, ex.MOTION_GATHER, [], 2))
+    assert mock.GgExecRecvTupleChunks(x.state, out, got) == 0, mock.GgExecLastError()
+    assert x.rows() == sent
+    x.end()
+
+
 def test_a_truncated_stream_is_refused(mock):
     eng = mock.mock_engine()
     stream, n, rows = partial_chunks(mock, eng, 0, 8124)
