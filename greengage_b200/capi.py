@@ -241,6 +241,8 @@ def dev_lib():
         L.gg_sort_rows.argtypes = [vp, C.POINTER(gg_sortkey), i32, i32, vp, vp, u64, vp]
         L.gg_sort_device.argtypes = [vp, C.POINTER(gg_sortkey), i32, i32, vp, vp, u64, vp, C.POINTER(i32)]
         L.gg_sort_datumrows.argtypes = [vp, C.POINTER(gg_sortkey), i32, i32, vp, u64, vp, C.POINTER(u64), C.POINTER(i32)]
+        L.gg_sort_datumrows_bounded.argtypes = [vp, C.POINTER(gg_sortkey), i32, i32, vp, u64, u64, vp, C.POINTER(u64), C.POINTER(i32)]
+        L.gg_sort_rows_bounded.argtypes = [vp, C.POINTER(gg_sortkey), i32, i32, vp, vp, u64, u64, vp, C.POINTER(u64)]
         L.gg_relation_attach_rows.argtypes = [vp, vp, u64, i32, C.POINTER(vp)]
         # device-resident aggregate rows and the NCCL interconnect
         L.gg_scanagg_groups.argtypes = [vp, C.POINTER(vp)]

@@ -12,7 +12,7 @@ import numpy as np
 from . import capi
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-T_SeqScan, T_Agg, T_Hash, T_HashJoin, T_Sort, T_Motion = 1, 2, 3, 4, 5, 6
+T_SeqScan, T_Agg, T_Hash, T_HashJoin, T_Sort, T_Motion, T_Limit = 1, 2, 3, 4, 5, 6, 7
 MOTION_GATHER, MOTION_HASH, MOTION_BROADCAST = 0, 1, 2
 GG_MAX_SORTKEYS = 4
 GG_MAX_OUTCOLS = capi.GG_MAX_KEYS + 3 * capi.GG_MAX_AGGS
@@ -51,6 +51,11 @@ class GgMotion(C.Structure):
     _fields_ = [("plan", GgPlan), ("motionType", C.c_int32), ("numHashCols", C.c_int32),
                 ("hashCol", C.c_int32 * capi.GG_MAX_KEYS), ("motionID", C.c_int32),
                 ("numSortCols", C.c_int32), ("sortKeys", capi.gg_sortkey * GG_MAX_SORTKEYS)]
+
+
+class GgLimit(C.Structure):
+    _fields_ = [("plan", GgPlan), ("hasOffset", C.c_int32), ("hasCount", C.c_int32), ("limitOffset", C.c_int64),
+                ("limitCount", C.c_int64)]
 
 
 class GgTupleTableSlot(C.Structure):
@@ -174,6 +179,14 @@ class PlanBuilder:
         n.plan.type, n.plan.qual, n.plan.lefttree, n.numCols = T_Sort, -1, _as_plan(child), len(keys)
         for i, k in enumerate(keys):
             n.keys[i] = k
+        return n
+
+    def limit(self, child, count=None, offset=None):
+        """LIMIT count OFFSET offset; None = LIMIT ALL / no OFFSET (the translator's evaluated constants)"""
+        n = self._keep(GgLimit())
+        n.plan.type, n.plan.qual, n.plan.lefttree = T_Limit, -1, _as_plan(child)
+        n.hasCount, n.limitCount = (0, 0) if count is None else (1, count)
+        n.hasOffset, n.limitOffset = (0, 0) if offset is None else (1, offset)
         return n
 
     def motion(self, child, motion_type, hash_cols=(), motion_id=1, merge_keys=()):

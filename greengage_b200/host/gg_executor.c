@@ -26,7 +26,15 @@
 int32_t gg_cdbhash_route(const int32_t *typids, const int64_t *vals, const int32_t *lens, const int32_t *isnull,
                          int nkeys, int nsegs);      /* gg_motion_host.c */
 
-enum { K_SCANAGG = 1, K_JOINAGG, K_AGGFINAL, K_SORT, K_MOTION, K_SCANROWS, K_HASH };
+enum { K_SCANAGG = 1, K_JOINAGG, K_AGGFINAL, K_SORT, K_MOTION, K_SCANROWS, K_HASH, K_LIMIT };
+
+#define GG_NO_BOUND UINT64_MAX
+
+/* The bounded sorts are referenced weakly, so this library still links and loads against a device library (or a stand-in for
+ * one) that lacks them.  Without them, a Limit over a Sort is refused at ExecInitNode with GG_ERR_UNSUPPORTED, and the caller
+ * keeps its CPU nodes for that subtree; no other sort takes their place. */
+#pragma weak gg_sort_rows_bounded
+#pragma weak gg_sort_datumrows_bounded
 
 struct GgPlanState {
 	int kind;
@@ -55,6 +63,7 @@ struct GgPlanState {
 	/* result set: filled on demand, then handed out row by row */
 	int done;                           /* pipeline has run */
 	int sort_runs;                      /* Sort over host rows: sorted runs the last execution merged (1: it fitted the operator's memory) */
+	uint64_t sort_bound;                /* Sort: rows the Limit above wants (SortState.bound, set by pass_down_bound); GG_NO_BOUND: all */
 	double instr_ntuples, instr_nloops; /* Instrumentation: tuples handed up, executions */
 	int rows_ready;                     /* host arrays below are filled */
 	int squelched;
@@ -105,6 +114,7 @@ const char *GgExecNodeKind(GgPlanState *s)
 		case K_MOTION: return "motion";
 		case K_SCANROWS: return "scanrows";
 		case K_HASH: return "hash";
+		case K_LIMIT: return "limit";
 	}
 	return "";
 }
@@ -487,10 +497,19 @@ static GgPlanState *init_node(GgPlan *node, GgEState *estate, int eflags, int de
 			GgSort *so = (GgSort *) node;
 			if (so->numCols < 1 || so->numCols > GG_MAX_SORTKEYS) { exec_fail(GG_ERR_UNSUPPORTED, "Sort with %d keys", so->numCols); goto fail; }
 			s->kind = K_SORT;
+			s->sort_bound = GG_NO_BOUND;
 			s->child = init_node(node->lefttree, estate, eflags, depth + 1);
 			if (!s->child) goto fail;
 			return s;
 		}
+		case T_GgLimit:
+			if (!node->lefttree) { exec_fail(GG_ERR_ARG, "Limit without a child"); goto fail; }
+			if (node->lefttree->type == T_GgSort && (!gg_sort_rows_bounded || !gg_sort_datumrows_bounded))
+			{ exec_fail(GG_ERR_UNSUPPORTED, "Limit over a Sort: the device library has no bounded sort"); goto fail; }
+			s->kind = K_LIMIT;
+			s->child = init_node(node->lefttree, estate, eflags, depth + 1);
+			if (!s->child) goto fail;
+			return s;
 		case T_GgMotion:
 		{
 			GgMotion *mo = (GgMotion *) node;
@@ -590,9 +609,10 @@ static int sort_row_cmp(const gg_sortkey *keys, int nkeys, int ncols, const int6
 
 typedef struct { uint64_t pos, end; } SortRun;         /* the run's head and its end, as indices into perm[] */
 
-/* perm[] = the sorted order of `n` rows: run by run through gg_sort_rows, then merged.  run_rows >= 1. */
+/* perm[] = the sorted order of `n` rows: run by run through gg_sort_rows, then merged.  run_rows >= 1.  With a bound (a Limit
+ * above), every run keeps only its first `bound` rows (gg_sort_rows_bounded) and the merge stops after `bound` rows. */
 static int sort_rows_external(gg_engine *eng, const gg_sortkey *keys, int nkeys, int ncols, const int64_t *values, const uint8_t *isnull,
-                              uint64_t n, uint64_t run_rows, uint64_t *perm, int *nruns_out)
+                              uint64_t n, uint64_t run_rows, uint64_t bound, uint64_t *perm, int *nruns_out)
 {
 	const uint64_t nruns = (n + run_rows - 1) / run_rows;
 	uint64_t *runperm, r, i, out = 0;
@@ -609,16 +629,23 @@ static int sort_rows_external(gg_engine *eng, const gg_sortkey *keys, int nkeys,
 	for (r = 0; r < nruns && rc == GG_OK; r++)
 	{
 		const uint64_t first = r * run_rows, len = first + run_rows <= n ? run_rows : n - first;
-		rc = gg_sort_rows(eng, keys, nkeys, ncols, values + first * (uint64_t) ncols, isnull + first * (uint64_t) ncols, len, runperm + first);
-		for (i = 0; i < len && rc == GG_OK; i++) runperm[first + i] += first;      /* row numbers of the whole input */
-		runs[r].pos = first; runs[r].end = first + len;
+		uint64_t kept = len;
+		if (bound < len)
+			rc = gg_sort_rows_bounded(eng, keys, nkeys, ncols, values + first * (uint64_t) ncols, isnull + first * (uint64_t) ncols, len, bound,
+			                          runperm + first, &kept);
+		else
+			rc = gg_sort_rows(eng, keys, nkeys, ncols, values + first * (uint64_t) ncols, isnull + first * (uint64_t) ncols, len, runperm + first);
+		for (i = 0; i < kept && rc == GG_OK; i++) runperm[first + i] += first;     /* row numbers of the whole input */
+		runs[r].pos = first; runs[r].end = first + kept;
 	}
 	if (rc == GG_OK)
 	{
 		/* build the heap of run heads, then pop the smallest head, advance its run, sift down: mergeonerun */
 		for (r = 0; r < nruns; r++)
 		{
-			uint32_t at = hn++;
+			uint32_t at;
+			if (runs[r].pos == runs[r].end) continue;
+			at = hn++;
 			heap[at] = (uint32_t) r;
 			while (at > 0)
 			{
@@ -629,7 +656,7 @@ static int sort_rows_external(gg_engine *eng, const gg_sortkey *keys, int nkeys,
 				at = up;
 			}
 		}
-		while (hn > 0)
+		while (hn > 0 && out < bound)
 		{
 			const uint32_t top = heap[0];
 			uint32_t at = 0;
@@ -672,10 +699,10 @@ static int sort_keys(gg_sortkey *keys, const gg_sortkey *plan_keys, int nkeys, c
 }
 
 /* the result of s = the host rows of src (s itself, or the node below) in the order of keys[]; with run_rows > 0 and more
- * rows than that, sorted externally and s->sort_runs counts the runs */
-static int sort_host_rows(GgPlanState *s, const GgPlanState *src, const gg_sortkey *keys, int nkeys, uint64_t run_rows)
+ * rows than that, sorted externally and s->sort_runs counts the runs.  With a bound, only the first `bound` rows of that order. */
+static int sort_host_rows(GgPlanState *s, const GgPlanState *src, const gg_sortkey *keys, int nkeys, uint64_t run_rows, uint64_t bound)
 {
-	const int64_t n = src->nrows;
+	const int64_t n = src->nrows > 0 && (uint64_t) src->nrows > bound ? (int64_t) bound : src->nrows;     /* rows of the result */
 	const int32_t ncols = src->ncols;
 	const size_t cells = (size_t) (n > 0 ? n : 1) * (size_t) ncols;
 	uint64_t *perm = malloc(8 * (size_t) (n > 0 ? n : 1));
@@ -683,11 +710,17 @@ static int sort_host_rows(GgPlanState *s, const GgPlanState *src, const gg_sortk
 	uint8_t *nl = malloc(cells);
 	int32_t *ln = malloc(4 * cells);
 	int64_t r;
+	uint64_t kept = 0;
 	int rc = GG_ERR_NOMEM;
 	if (perm && v && nl && ln)
-		rc = run_rows && (uint64_t) n > run_rows
-		   ? sort_rows_external(s->estate->engine, keys, nkeys, ncols, src->values, src->isnull, (uint64_t) n, run_rows, perm, &s->sort_runs)
-		   : gg_sort_rows(s->estate->engine, keys, nkeys, ncols, src->values, src->isnull, (uint64_t) n, perm);
+	{
+		if (run_rows && (uint64_t) src->nrows > run_rows && bound > run_rows)
+			rc = sort_rows_external(s->estate->engine, keys, nkeys, ncols, src->values, src->isnull, (uint64_t) src->nrows, run_rows, bound, perm, &s->sort_runs);
+		else if (n < src->nrows)
+			rc = gg_sort_rows_bounded(s->estate->engine, keys, nkeys, ncols, src->values, src->isnull, (uint64_t) src->nrows, bound, perm, &kept);
+		else
+			rc = gg_sort_rows(s->estate->engine, keys, nkeys, ncols, src->values, src->isnull, (uint64_t) n, perm);
+	}
 	if (rc != GG_OK)
 	{
 		exec_fail(rc, "%s", rc == GG_ERR_NOMEM ? "out of memory" : gg_last_error());
@@ -797,6 +830,12 @@ static int run_rows_node(GgPlanState *s)
 	return 0;
 }
 
+/* the device buffer that holds a rows node's datum rows */
+static gg_relation *rows_buffer(const GgPlanState *s)
+{
+	return s->rows_recv && s->rows_nsegs > 1 ? s->rows_recv : s->rows_send;
+}
+
 /* device rows -> host result arrays (only when a rows node sits at the top of what the caller drives) */
 static int rows_to_host(GgPlanState *s)
 {
@@ -812,7 +851,7 @@ static int rows_to_host(GgPlanState *s)
 		uint64_t live = 0;
 		buf = malloc((size_t) nb * GG_BLCKSZ);
 		if (!buf) { exec_fail(GG_ERR_NOMEM, "out of memory"); return -1; }
-		rc = gg_relation_read(s->rows_recv && s->rows_nsegs > 1 ? s->rows_recv : s->rows_send, 0, buf, nb);
+		rc = gg_relation_read(rows_buffer(s), 0, buf, nb);
 		if (rc != GG_OK) { free(buf); exec_fail(rc, "%s", gg_last_error()); return -1; }
 		for (r = 0; r < n; r++)
 		{
@@ -975,7 +1014,7 @@ static int motion_host_path(GgPlanState *s, int child_failed)
 		 * the Sort node's (tuplesort_mk.c:2816), ties in unspecified order as in the reference's merge */
 		gg_sortkey keys[GG_MAX_SORTKEYS];
 		if (mo->numSortCols > GG_MAX_SORTKEYS) { exec_fail(GG_ERR_UNSUPPORTED, "Motion with %d merge keys", mo->numSortCols); return -1; }
-		if (sort_keys(keys, mo->sortKeys, mo->numSortCols, s, "Motion merge") || sort_host_rows(s, s, keys, mo->numSortCols, 0)) return -1;
+		if (sort_keys(keys, mo->sortKeys, mo->numSortCols, s, "Motion merge") || sort_host_rows(s, s, keys, mo->numSortCols, 0, GG_NO_BOUND)) return -1;
 	}
 	s->rows_ready = 1;
 	return 0;
@@ -1077,7 +1116,8 @@ static int run_sort(GgPlanState *s)
 		/* the input is datum rows on the device (a row-producing SeqScan, or the Motion over one): sort them where they
 		 * are; the sorted rows stay on the device for the node above, or come to the host once, at the top */
 		const uint64_t W = 1 + (uint64_t) ch->rows_ncols;
-		const uint64_t nb = (ch->rows_n * W * 8 + 64 + GG_BLCKSZ - 1) / GG_BLCKSZ;
+		const uint64_t nout = ch->rows_n < s->sort_bound ? ch->rows_n : s->sort_bound;
+		const uint64_t nb = (nout * W * 8 + 64 + GG_BLCKSZ - 1) / GG_BLCKSZ;
 		uint64_t live = 0;
 		drop_device_results(s);
 		if (s->rows_send && gg_relation_nblocks(s->rows_send) < nb) { gg_relation_free(s->rows_send); s->rows_send = NULL; }
@@ -1086,8 +1126,13 @@ static int run_sort(GgPlanState *s)
 			rc = gg_relation_create(es->engine, nb, &s->rows_send);
 			if (rc != GG_OK) { exec_fail(rc, "Sort result: %s", gg_last_error()); return -1; }
 		}
-		rc = gg_sort_datumrows(es->engine, keys, so->numCols, ch->rows_ncols, gg_relation_device_ptr(ch->rows_rel), ch->rows_n,
-		                       gg_relation_device_ptr(s->rows_send), &live, NULL);
+		/* bounded (a Limit above): only the first sort_bound rows of the order are selected, sorted and written */
+		if (s->sort_bound != GG_NO_BOUND)
+			rc = gg_sort_datumrows_bounded(es->engine, keys, so->numCols, ch->rows_ncols, gg_relation_device_ptr(ch->rows_rel), ch->rows_n,
+			                               s->sort_bound, gg_relation_device_ptr(s->rows_send), &live, NULL);
+		else
+			rc = gg_sort_datumrows(es->engine, keys, so->numCols, ch->rows_ncols, gg_relation_device_ptr(ch->rows_rel), ch->rows_n,
+			                       gg_relation_device_ptr(s->rows_send), &live, NULL);
 		if (rc != GG_OK) { exec_fail(rc, "%s", gg_last_error()); return -1; }
 		s->rows_n = live; s->rows_ncols = ch->rows_ncols; s->rows_nsegs = 1;
 		s->ncols = ch->ncols;
@@ -1104,7 +1149,114 @@ static int run_sort(GgPlanState *s)
 	run_rows = es->es_operator_mem ? es->es_operator_mem / (rowbytes ? rowbytes : 1) : 0;
 	if (run_rows && run_rows < 256) run_rows = 256;
 	s->sort_runs = 1;
-	if (sort_host_rows(s, ch, keys, so->numCols, run_rows)) return -1;
+	/* bounded: when the bound's rows fit the operator's memory, one bounded sort and no runs at all (tuplesort_mk's bounded
+	 * heap never spills); otherwise each run keeps its first `bound` rows and the merge stops there */
+	if (sort_host_rows(s, ch, keys, so->numCols, run_rows, s->sort_bound)) return -1;
+	s->rows_ready = 1;
+	return 0;
+}
+
+/* ---- Limit (nodeLimit.c): forward-only; the window [offset, offset + count) of the child's rows as host rows ---- */
+
+/* s's result = live datum rows [skip, skip + take) of ch, copied from the device a few 32 KB blocks at a time: only the leading
+ * blocks that hold them, never the whole buffer.  *pulled: live rows of ch read (skip + the rows taken). */
+static int rows_window_to_host(GgPlanState *s, const GgPlanState *ch, uint64_t skip, uint64_t take, uint64_t *pulled)
+{
+	const uint64_t W = 1 + (uint64_t) ch->rows_ncols;
+	const uint64_t total_nb = (ch->rows_n * W * 8 + GG_BLCKSZ - 1) / GG_BLCKSZ;
+	const uint64_t need = skip + take < skip ? UINT64_MAX : skip + take;
+	gg_relation *src = rows_buffer(ch);
+	uint64_t *buf = NULL, have_nb = 0, r = 0, live = 0, out = 0;
+	int c, rc;
+	const uint64_t cap = take < (uint64_t) ch->rows_n ? take : (uint64_t) ch->rows_n;
+	if (alloc_result(s, (int64_t) cap, ch->rows_ncols)) { exec_fail(GG_ERR_NOMEM, "out of memory"); return -1; }
+	while (r < ch->rows_n && live < need)
+	{
+		/* every block so far held rows; ask for enough new blocks to hold the rows still wanted if none of them were dead */
+		const uint64_t rows_wanted = need - live < ch->rows_n - r ? need - live : ch->rows_n - r;
+		uint64_t want_nb = ((r + rows_wanted) * W * 8 + GG_BLCKSZ - 1) / GG_BLCKSZ;
+		uint64_t *nbuf;
+		if (want_nb <= have_nb) want_nb = have_nb + 1;
+		if (want_nb > total_nb) want_nb = total_nb;
+		nbuf = realloc(buf, (size_t) want_nb * GG_BLCKSZ);
+		if (!nbuf) { free(buf); exec_fail(GG_ERR_NOMEM, "out of memory"); return -1; }
+		buf = nbuf;
+		rc = gg_relation_read(src, have_nb, (uint8_t *) buf + have_nb * GG_BLCKSZ, want_nb - have_nb);
+		if (rc != GG_OK) { free(buf); exec_fail(rc, "%s", gg_last_error()); return -1; }
+		have_nb = want_nb;
+		for (; r < ch->rows_n && (r + 1) * W * 8 <= have_nb * GG_BLCKSZ && live < need; r++)
+		{
+			if (buf[r * W] & GG_DATUMROW_DEAD) continue;            /* a slot the sending kernel claimed and did not fill */
+			if (live++ < skip) continue;
+			for (c = 0; c < ch->rows_ncols; c++)
+			{
+				const uint64_t v = buf[r * W + 1 + c];
+				s->values[out * ch->rows_ncols + c] = (int64_t) v;
+				s->isnull[out * ch->rows_ncols + c] = (uint8_t) ((buf[r * W] >> c) & 1);
+				if (is_string_type(ch->typid[c])) s->lens[out * ch->rows_ncols + c] = packed_len(v);
+			}
+			out++;
+		}
+	}
+	free(buf);
+	s->nrows = (int64_t) out;
+	*pulled = live;
+	return 0;
+}
+
+static int run_limit(GgPlanState *s)
+{
+	const GgLimit *lp = (const GgLimit *) s->plan;
+	GgPlanState *ch = s->child;
+	const int64_t offset = lp->hasOffset ? lp->limitOffset : 0;
+	const int64_t count = lp->hasCount ? lp->limitCount : 0;
+	uint64_t skip, take, pulled = 0;
+	/* recompute_limits (nodeLimit.c:258), at the first run and at every ReScan */
+	if (offset < 0) { exec_fail(GG_ERR_ARG, "OFFSET must not be negative"); return -1; }
+	if (count < 0) { exec_fail(GG_ERR_ARG, "LIMIT must not be negative"); return -1; }
+	/* pass_down_bound (nodeLimit.c:345): a Sort below needs only count + offset rows; no bound for LIMIT ALL, a sum that
+	 * overflows, or one tuplesort_set_bound would not take (tuplesort_mk.c:1011) */
+	if (ch->kind == K_SORT)
+	{
+		const int64_t needed = (int64_t) ((uint64_t) count + (uint64_t) offset);
+		ch->sort_bound = (!lp->hasCount || needed < 0 || needed > INT32_MAX / 2) ? GG_NO_BOUND : (uint64_t) needed;
+	}
+	if (lp->hasCount && count <= 0)
+	{
+		/* an empty window: the child never runs; the squelch still runs a Motion below whose peers are in the exchange */
+		GgExecSquelchNode(ch);
+		inherit_layout(s, ch);
+		if (alloc_result(s, 0, s->ncols > 0 ? s->ncols : 1)) { exec_fail(GG_ERR_NOMEM, "out of memory"); return -1; }
+		s->nonreceiver = ch->nonreceiver;
+		s->rows_ready = 1;
+		return 0;
+	}
+	if (run_child(s)) return -1;
+	s->nonreceiver = ch->nonreceiver;
+	inherit_layout(s, ch);
+	skip = (uint64_t) offset;
+	take = lp->hasCount ? (uint64_t) count : UINT64_MAX;
+	if (ch->rows_rel && !ch->rows_ready)
+	{
+		if (rows_window_to_host(s, ch, skip, take, &pulled)) return -1;
+	}
+	else
+	{
+		uint64_t n, first, len;
+		if (ensure_rows(ch)) return -1;
+		n = ch->nrows > 0 ? (uint64_t) ch->nrows : 0;
+		first = skip < n ? skip : n;
+		len = n - first < take ? n - first : take;
+		if (alloc_result(s, (int64_t) len, ch->ncols)) { exec_fail(GG_ERR_NOMEM, "out of memory"); return -1; }
+		memcpy(s->values, ch->values + first * (uint64_t) ch->ncols, 8 * (size_t) len * (size_t) ch->ncols);
+		memcpy(s->isnull, ch->isnull + first * (uint64_t) ch->ncols, (size_t) len * (size_t) ch->ncols);
+		memcpy(s->lens, ch->lens + first * (uint64_t) ch->ncols, 4 * (size_t) len * (size_t) ch->ncols);
+		pulled = first + len;
+	}
+	/* the rows ExecLimit pulled through the child's ExecProcNode, for the child's Instrumentation */
+	ch->instr_ntuples += (double) pulled;
+	/* the window is complete: the node below will not be read again (ExecLimit, nodeLimit.c:239-247) */
+	GgExecSquelchNode(ch);
 	s->rows_ready = 1;
 	return 0;
 }
@@ -1163,6 +1315,7 @@ static int run_node(GgPlanState *s)
 		case K_AGGFINAL: rc = run_final_agg(s); break;
 		case K_SORT: rc = run_sort(s); break;
 		case K_MOTION: rc = run_motion(s); break;
+		case K_LIMIT: rc = run_limit(s); break;
 		default:
 			exec_fail(GG_ERR_ARG, "bad plan state");
 			return -1;
@@ -1527,6 +1680,11 @@ GgTupleTableSlot *GgExecSort(GgPlanState *node) { return GgExecProcNode(node); }
 void GgExecEndSort(GgPlanState *node) { GgExecEndNode(node); }
 int GgExecReScanSort(GgPlanState *node) { return GgExecReScan(node); }
 void GgExecSquelchSort(GgPlanState *node) { GgExecSquelchNode(node); }
+GgPlanState *GgExecInitLimit(GgLimit *node, GgEState *estate, int eflags) { return init_tagged(&node->plan, T_GgLimit, estate, eflags); }
+GgTupleTableSlot *GgExecLimit(GgPlanState *node) { return GgExecProcNode(node); }
+void GgExecEndLimit(GgPlanState *node) { GgExecEndNode(node); }
+int GgExecReScanLimit(GgPlanState *node) { return GgExecReScan(node); }
+void GgExecSquelchLimit(GgPlanState *node) { GgExecSquelchNode(node); }
 /* ExecSortMarkPos / ExecSortRestrPos (nodeSort.c:444,462): the sorted result is materialised, so a position is an index */
 void GgExecSortMarkPos(GgPlanState *node) { if (node && node->done) node->markpos = node->next; }
 void GgExecSortRestrPos(GgPlanState *node) { if (node && node->done) node->next = node->markpos; }

@@ -7,7 +7,7 @@
  *     ExecEndNode    src/backend/executor/execProcnode.c:1315
  *     ExecReScan     src/backend/executor/execAmi.c:76
  *     ExecSquelchNode src/backend/executor/execAmi.c:641
- * with the node types of the accelerated path (plannodes.h): SeqScan, Agg, Hash, HashJoin, Sort, Motion.
+ * with the node types of the accelerated path (plannodes.h): SeqScan, Agg, Hash, HashJoin, Sort, Motion, Limit.
  * Names keep the reference's, prefixed Gg.  The plan tree is what the Postgres-side translator of
  * INTEGRATION.md §2 builds from the real Plan tree; expressions live in one gg_exprpool.
  *
@@ -35,7 +35,8 @@ typedef enum GgNodeTag {            /* nodes/nodes.h NodeTag, the accelerated su
 	T_GgHash,
 	T_GgHashJoin,
 	T_GgSort,
-	T_GgMotion
+	T_GgMotion,
+	T_GgLimit
 } GgNodeTag;
 
 typedef enum GgMotionType {         /* plannodes.h MotionType */
@@ -99,6 +100,15 @@ typedef struct GgMotion {
 	int32_t numSortCols;
 	gg_sortkey sortKeys[GG_MAX_SORTKEYS];
 } GgMotion;
+
+/* Limit (plannodes.h Limit): limitOffset / limitCount are the constants the translator evaluated the expressions to.
+ * hasCount == 0: LIMIT ALL; hasOffset == 0: OFFSET 0.  Forward scans only.  The node's result is the window as host rows; a
+ * Sort directly below it is told how many rows are wanted (pass_down_bound, nodeLimit.c:345) and sorts only those. */
+typedef struct GgLimit {
+	GgPlan plan;
+	int32_t hasOffset, hasCount;
+	int64_t limitOffset, limitCount;
+} GgLimit;
 
 /* TupleTableSlot holding a virtual tuple (tuptable.h:117-175): Datums + null flags */
 typedef struct GgTupleTableSlot {
@@ -168,7 +178,7 @@ int  GgExecReScan(GgPlanState *node);
 void GgExecSquelchNode(GgPlanState *node);
 const char *GgExecLastError(void);
 int  GgExecLastErrorCode(void);                /* GG_ERR_* of the failure, GG_OK if none */
-/* introspection: which device pipeline a state node was fused into ("scanagg", "joinagg", "sort", "motion") */
+/* introspection: which device pipeline a state node was fused into ("scanagg", "joinagg", "sort", "motion", "limit", ...) */
 const char *GgExecNodeKind(GgPlanState *node);
 /* where a node that has run keeps its result: "device-groups" (aggregate rows as group records), "device-rows" (datum rows)
  * or "host" (Datum arrays); "" before it has run */
@@ -217,6 +227,13 @@ GgTupleTableSlot *GgExecMotion(GgPlanState *node);
 void GgExecEndMotion(GgPlanState *node);
 int  GgExecReScanMotion(GgPlanState *node);
 void GgExecSquelchMotion(GgPlanState *node);
+/* nodeLimit.h:19-23.  LIMIT / OFFSET must not be negative (GG_ERR_ARG, the reference's message); an empty window never runs
+ * the child, and a window that ends squelches it (ExecLimit, nodeLimit.c:239-247) */
+GgPlanState *GgExecInitLimit(GgLimit *node, GgEState *estate, int eflags);
+GgTupleTableSlot *GgExecLimit(GgPlanState *node);
+void GgExecEndLimit(GgPlanState *node);
+int  GgExecReScanLimit(GgPlanState *node);
+void GgExecSquelchLimit(GgPlanState *node);
 void GgExecSortMarkPos(GgPlanState *node);      /* nodeSort.c:444 ExecSortMarkPos */
 void GgExecSortRestrPos(GgPlanState *node);     /* nodeSort.c:462 ExecSortRestrPos */
 GgPlanState *GgExecInitHashJoin(GgHashJoin *node, GgEState *estate, int eflags);

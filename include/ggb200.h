@@ -194,6 +194,15 @@ int  gg_sort_device(gg_engine *e, const gg_sortkey *keys, int nkeys, int ncols, 
  * keys[].col counts the row's columns from 0. */
 int  gg_sort_datumrows(gg_engine *e, const gg_sortkey *keys, int nkeys, int ncols, const void *dev_rows, uint64_t n,
                        void *dev_out_rows, uint64_t *nlive, int *passes);
+/* Bounded Sort (tuplesort_set_bound, tuplesort_mk.c:1000; a Limit above wants only the first `bound` rows): the first
+ * min(bound, live) rows of what gg_sort_datumrows returns for the same input, byte for byte, in dev_out_rows; *nout = that
+ * count.  A radix select on the first key keeps the rows that can be among them, in input order, and only those are sorted
+ * (DESIGN §4.4).  bound == 0 launches nothing.  passes: histogram passes of the selection plus radix passes of the sort. */
+int  gg_sort_datumrows_bounded(gg_engine *e, const gg_sortkey *keys, int nkeys, int ncols, const void *dev_rows, uint64_t n,
+                               uint64_t bound, void *dev_out_rows, uint64_t *nout, int *passes);
+/* the same for host rows: host_perm receives the first min(bound, n) entries of gg_sort_rows's permutation; *nperm = count */
+int  gg_sort_rows_bounded(gg_engine *e, const gg_sortkey *keys, int nkeys, int ncols, const int64_t *host_rows,
+                          const uint8_t *host_nulls, uint64_t n, uint64_t bound, uint64_t *host_perm, uint64_t *nperm);
 
 /* ---- Motion ----
  * Sending side of a Redistribute Motion (nodeMotion.c:1481-1687, cdbhash.c:173-287) on the device: evaluates the
