@@ -238,6 +238,11 @@ def dev_lib():
         L.gg_joinagg_stats.argtypes = [vp, C.POINTER(u64), C.POINTER(u64), C.POINTER(C.c_float), C.POINTER(C.c_float)]
         L.gg_joinagg_free.argtypes = [vp]
         L.gg_joinagg_free.restype = None
+        L.gg_joinrows_create.argtypes = [vp, C.POINTER(gg_scan), C.POINTER(gg_scan), C.POINTER(gg_hashjoin), C.POINTER(C.c_int32), i32,
+                                         C.POINTER(gg_exprpool), C.POINTER(vp)]
+        L.gg_joinagg_rows.argtypes = [vp, C.POINTER(vp), C.POINTER(u64), C.POINTER(u64)]
+        L.gg_debug_disasm_joinrows.argtypes = [C.POINTER(gg_scan), C.POINTER(gg_scan), C.POINTER(gg_hashjoin), C.POINTER(C.c_int32), i32,
+                                               C.POINTER(gg_exprpool), C.c_char_p, i32]
         L.gg_sort_rows.argtypes = [vp, C.POINTER(gg_sortkey), i32, i32, vp, vp, u64, vp]
         L.gg_sort_device.argtypes = [vp, C.POINTER(gg_sortkey), i32, i32, vp, vp, u64, vp, C.POINTER(i32)]
         L.gg_sort_datumrows.argtypes = [vp, C.POINTER(gg_sortkey), i32, i32, vp, u64, vp, C.POINTER(u64), C.POINTER(i32)]

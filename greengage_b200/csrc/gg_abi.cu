@@ -335,6 +335,22 @@ extern "C" int gg_debug_disasm_join(const gg_scan *outer, const gg_scan *inner, 
 	return n;
 }
 
+/* debugging aid: the build and probe programs of a HashJoin with a target list */
+extern "C" int gg_debug_disasm_joinrows(const gg_scan *outer, const gg_scan *inner, const gg_hashjoin *hj, const int32_t *targets,
+                                        int ntargets, const gg_exprpool *pool, char *buf, int cap)
+{
+	std::vector<ggp_joinprog> jpbuf(1);
+	ggp_joinprog &jp = jpbuf[0];
+	char msg[256];
+	int rc = ggp_compile_joinrows(outer, inner, hj, targets, ntargets, pool, &jp, msg, sizeof msg);
+	if (rc != GG_OK) { gg_set_error("%s", msg); return rc; }
+	int n = snprintf(buf, (size_t) cap, "-- build (payload %d)\n", jp.npayload);
+	n += ggp_disasm(&jp.build, buf + n, cap - n);
+	n += snprintf(buf + n, (size_t) (cap - n), "-- probe (per-match segment from pc %d)\n", jp.probe_pc);
+	n += ggp_disasm(&jp.probe, buf + n, cap - n);
+	return n;
+}
+
 /* debugging aid: the plan-specialised source gg_jit.cpp would compile for this plan and kernel variant */
 #include "gg_jit.h"
 extern "C" int gg_debug_jit_source(const gg_scan *scan, const gg_agg *agg, const gg_exprpool *pool, int mode, int threads,

@@ -996,10 +996,46 @@ static int join_keytype(int32_t outer, int32_t inner)
 	return 0;
 }
 
-/* HashJoin + Agg: see ggp_joinprog in gg_program.h.  Stands where ExecInitHashJoin / ExecInitHash prepare
- * hj_OuterHashKeys / hashkeys and the hash functions (nodeHashjoin.c:540-750, nodeHash.c:270-450). */
-int ggp_compile_join(const gg_scan *outer, const gg_scan *inner, const gg_hashjoin *hj, const gg_agg *agg,
-                     const gg_exprpool *pool, ggp_joinprog *jp, ggp_aggmap *aggmap, char *err, int errlen)
+/* does the expression at `root` (a validated pool) read a column of side `varno` */
+static bool refs_side(const gg_exprpool *pool, int root, int varno)
+{
+	const gg_expr &e = pool->nodes[root];
+	if (e.kind == GG_E_VAR) return e.varno == varno;
+	const int n = e.kind == GG_E_CONST ? 0 : (e.nargs < 2 ? e.nargs : 2);
+	for (int k = 0; k < n; k++)
+		if (e.args[k] >= 0 && e.args[k] < root && refs_side(pool, e.args[k], varno)) return true;     /* children come first */
+	return false;
+}
+
+/* the per-match piece of a join with a target list: claim a row, then one output column per target (what ggp_compile_motion
+ * gives its payload, without the hash keys) */
+static void compile_rows_part(Ctx &c, const int32_t *targets, int ntargets)
+{
+	ggp_program *prog = c.prog;
+	emit(c, GGP_NOP);
+	prog->code[prog->ncode - 1].flags |= GGP_F_GROUP;
+	for (int p = 0; p < ntargets && !c.failed; p++)
+	{
+		const int32_t t = c.pool->nodes[targets[p]].rettype;
+		if (t == GG_NUMERICOID) { fail(c, "join target %d: numeric columns do not travel as datum rows yet", p); break; }
+		if (!loadtype_of(t)) { fail(c, "join target %d: type %d not supported", p, t); break; }
+		ggp_op *o = gen_value(c, targets[p]);
+		if (c.failed) break;
+		if (o->flags & (GGP_F_OUT | GGP_F_GROUP)) { emit(c, GGP_NOP); o = &prog->code[prog->ncode - 1]; }
+		o->flags |= GGP_F_OUT;
+		o->out = (uint8_t) p;
+	}
+	emit(c, GGP_END);
+	prog->nkeys = 0;
+	prog->nslots = ntargets;
+	prog->priv_ok = 0;
+}
+
+/* HashJoin + Agg (agg != nullptr), or HashJoin with a target list (agg == nullptr): see ggp_joinprog in gg_program.h.  Stands
+ * where ExecInitHashJoin / ExecInitHash prepare hj_OuterHashKeys / hashkeys and the hash functions (nodeHashjoin.c:540-750,
+ * nodeHash.c:270-450). */
+static int compile_join(const gg_scan *outer, const gg_scan *inner, const gg_hashjoin *hj, const gg_agg *agg, const int32_t *targets,
+                        int ntargets, const gg_exprpool *pool, ggp_joinprog *jp, ggp_aggmap *aggmap, char *err, int errlen)
 {
 	Ctx c;
 	memset(jp, 0, sizeof *jp);
@@ -1007,6 +1043,7 @@ int ggp_compile_join(const gg_scan *outer, const gg_scan *inner, const gg_hashjo
 	c.pool = pool; c.err = err; c.errlen = errlen;
 	if (err && errlen) err[0] = 0;
 	if (hj->nkeys < 1 || hj->nkeys > 2) { fail(c, "hash join with %d keys not supported (1 or 2)", hj->nkeys); return GG_ERR_UNSUPPORTED; }
+	if (!agg && (ntargets < 1 || ntargets > 16)) { fail(c, "join projecting %d columns (1..16 travel as datum rows)", ntargets); return GG_ERR_UNSUPPORTED; }
 	{
 		Roots roots;
 		if (!valid_header(c, pool, &outer->desc, &inner->desc)) return GG_ERR_ARG;
@@ -1018,7 +1055,10 @@ int ggp_compile_join(const gg_scan *outer, const gg_scan *inner, const gg_hashjo
 			roots.add(c, pool, hj->outerkey[k], false, "outer join key");
 			roots.add(c, pool, hj->innerkey[k], false, "inner join key");
 		}
-		if (!add_agg_roots(c, agg, pool, roots) || !roots.ok || !valid_nodes(c, pool, &outer->desc, &inner->desc, roots)) return GG_ERR_ARG;
+		if (agg) { if (!add_agg_roots(c, agg, pool, roots)) return GG_ERR_ARG; }
+		else
+			for (int p = 0; p < ntargets; p++) roots.add(c, pool, targets[p], false, "join target");
+		if (!roots.ok || !valid_nodes(c, pool, &outer->desc, &inner->desc, roots)) return GG_ERR_ARG;
 	}
 	switch (hj->jointype)
 	{
@@ -1029,6 +1069,11 @@ int ggp_compile_join(const gg_scan *outer, const gg_scan *inner, const gg_hashjo
 			fail(c, "join type %d not supported", hj->jointype);
 			return GG_ERR_UNSUPPORTED;
 	}
+	/* a semi / anti join returns outer rows only (the matched inner row is not part of its result) */
+	if (!agg && (hj->jointype == GG_JOIN_SEMI || hj->jointype == GG_JOIN_ANTI || hj->jointype == GG_JOIN_LASJ_NOTIN))
+		for (int p = 0; p < ntargets; p++)
+			if (refs_side(pool, targets[p], 1))
+			{ fail(c, "join target %d reads an inner column: a semi or anti join returns outer rows only", p); return GG_ERR_UNSUPPORTED; }
 	/* a side that can come back null-extended makes every expression above the join nullable */
 	const bool nullext = hj->jointype != GG_JOIN_INNER && hj->jointype != GG_JOIN_SEMI;
 	jp->nkeys = hj->nkeys;
@@ -1066,7 +1111,7 @@ int ggp_compile_join(const gg_scan *outer, const gg_scan *inner, const gg_hashjo
 		if (!c.failed) o->flags |= GGP_F_FILTER;
 	}
 	if (nullext) jp->probe.nullable = 1;
-	if (!c.failed) compile_agg_part(c, agg, aggmap);
+	if (!c.failed) { if (agg) compile_agg_part(c, agg, aggmap); else compile_rows_part(c, targets, ntargets); }
 	jp->npayload = innerside.ncols;
 	if (nullext) { jp->probe.nullable = 1; jp->probe.priv_ok = 0; }
 
@@ -1118,6 +1163,18 @@ int ggp_compile_join(const gg_scan *outer, const gg_scan *inner, const gg_hashjo
 	for (int k = 0; k < hj->nkeys; k++) jp->build.keytype[k] = jp->keytype[k];
 	if (c.failed || b.failed) return GG_ERR_UNSUPPORTED;
 	return GG_OK;
+}
+
+int ggp_compile_join(const gg_scan *outer, const gg_scan *inner, const gg_hashjoin *hj, const gg_agg *agg,
+                     const gg_exprpool *pool, ggp_joinprog *jp, ggp_aggmap *aggmap, char *err, int errlen)
+{
+	return compile_join(outer, inner, hj, agg, nullptr, 0, pool, jp, aggmap, err, errlen);
+}
+
+int ggp_compile_joinrows(const gg_scan *outer, const gg_scan *inner, const gg_hashjoin *hj, const int32_t *targets, int ntargets,
+                         const gg_exprpool *pool, ggp_joinprog *jp, char *err, int errlen)
+{
+	return compile_join(outer, inner, hj, nullptr, targets, ntargets, pool, jp, nullptr, err, errlen);
 }
 
 /* Redistribute Motion (nodeMotion.c:1481-1687): which tuples go where, and what travels */

@@ -2,7 +2,8 @@
  * gg_join.cu — Hash / HashJoin (+ the Agg above): the build kernel and the probe into the general HashAggregate (interpreter
  * path), and the host pipeline behind gg_joinagg_* (include/ggb200.h).  The probe side IS a gg_scanagg pipeline (gg_pipeline.h)
  * whose row program has a per-match piece; everything after the probe (merge, fetch, escalation to the general HashAggregate)
- * is shared, and gg_scanagg.cu launches its kernels.
+ * is shared, and gg_scanagg.cu launches its kernels.  A join with a target list (gg_joinrows_create) is the same pipeline whose
+ * probe writes every joined row as a datum row instead (MODE_PART with JOIN = true: JoinRowSink).
  */
 #include "gg_pipeline.h"
 #include "gg_groups.h"
@@ -21,6 +22,13 @@ __global__ void __launch_bounds__(256, 2)
 gg_joinhash_kernel(const __grid_constant__ ggp_program P, const ScanAggParams prm)
 {
 	scanagg_body<MODE_HASH, DynPlan, true>(P, prm);
+}
+
+/* probe writing the joined rows of a join with a target list */
+__global__ void __launch_bounds__(256, 2)
+gg_joinrows_kernel(const __grid_constant__ ggp_program P, const ScanAggParams prm)
+{
+	scanagg_body<MODE_PART, DynPlan, true>(P, prm);
 }
 
 /* upper bound on the inner rows = line pointers of the pages (exact for a freshly loaded relation) */
@@ -107,12 +115,19 @@ struct gg_joinagg {
 	uint64_t ocap = 0, icap = 0;                             /* rows per region */
 	std::vector<uint64_t> ocounts, icounts;
 	float part_ms = 0;
+	/* a join with a target list (gg_joinrows_create): the probe writes its rows here instead of feeding `agg` (all zero) */
+	int ntargets = 0;
+	int32_t targets[16];
+	gg_relation *rows_buf = nullptr;            /* owned: datum rows of 1 + ntargets words, probe->mo.cap of them */
+	unsigned long long *d_rowcur = nullptr;     /* probe->mo.cursor: rows claimed, counted on past the capacity */
+	gg_relation *rows_view = nullptr;           /* what gg_joinagg_rows handed out (until reset / free) */
+	uint64_t rows_n = 0, rows_live = 0;
 };
 
-int gg_joinagg_create(gg_engine *e, const gg_scan *outer, const gg_scan *inner, const gg_hashjoin *hj,
-                      const gg_agg *agg, const gg_exprpool *pool, gg_joinagg **out)
+/* agg == nullptr: a join with a target list */
+static int joinagg_create(gg_engine *e, const gg_scan *outer, const gg_scan *inner, const gg_hashjoin *hj, const gg_agg *agg,
+                          const int32_t *targets, int ntargets, const gg_exprpool *pool, gg_joinagg **out)
 {
-	if (!e || !outer || !inner || !hj || !agg || !pool || !out) return GG_ERR_ARG;
 	*out = nullptr;
 	GG_CUDA(cudaSetDevice(e->device));
 	gg_joinagg *j = new gg_joinagg();
@@ -120,11 +135,14 @@ int gg_joinagg_create(gg_engine *e, const gg_scan *outer, const gg_scan *inner, 
 	gg_scanagg *p = new gg_scanagg();
 	p->eng = e;
 	p->scan = *outer;
-	p->agg = *agg;
+	memset(&p->agg, 0, sizeof p->agg);
+	if (agg) p->agg = *agg;
 	p->pool = *pool;
 	p->is_join = true;
+	p->join_rows = agg == nullptr;
 	char msg[256];
-	int rc = ggp_compile_join(outer, inner, hj, agg, pool, &j->jp, p->aggmap, msg, sizeof msg);
+	int rc = agg ? ggp_compile_join(outer, inner, hj, agg, pool, &j->jp, p->aggmap, msg, sizeof msg)
+	             : ggp_compile_joinrows(outer, inner, hj, targets, ntargets, pool, &j->jp, msg, sizeof msg);
 	if (rc != GG_OK) { gg_set_error("%s", msg); delete p; delete j; return rc; }
 	p->prog = j->jp.probe;
 	p->join_probe_pc = j->jp.probe_pc;
@@ -132,7 +150,15 @@ int gg_joinagg_create(gg_engine *e, const gg_scan *outer, const gg_scan *inner, 
 	if (p->prog.nullable) p->prog.priv_ok = 0;
 	rc = scanagg_finish_create(p, &j->probe);
 	if (rc) { delete j; return rc; }
-	j->outer_scan = *outer; j->inner_scan = *inner; j->hj = *hj; j->agg = *agg; j->pool = *pool;
+	j->outer_scan = *outer; j->inner_scan = *inner; j->hj = *hj; j->agg = p->agg; j->pool = *pool;
+	if (!agg)
+	{
+		j->ntargets = ntargets;
+		memcpy(j->targets, targets, sizeof(int32_t) * (size_t) ntargets);
+		GG_CUDA(cudaMalloc((void **) &j->d_rowcur, sizeof(unsigned long long)));
+		GG_CUDA(cudaMemsetAsync(j->d_rowcur, 0, sizeof(unsigned long long), e->stream));
+		j->probe->mo.cursor = j->d_rowcur;
+	}
 	GG_CUDA(cudaMalloc((void **) &j->d_cnt, 4 * sizeof(unsigned long long)));      /* line pointers | nbuilt[0..2] (JoinTable) */
 	GG_CUDA(cudaMalloc((void **) &j->d_buildcnt, 3 * sizeof(unsigned long long)));      /* rows scanned | passed | error flags */
 	GG_CUDA(cudaEventCreate(&j->ev0));
@@ -141,11 +167,65 @@ int gg_joinagg_create(gg_engine *e, const gg_scan *outer, const gg_scan *inner, 
 	return GG_OK;
 }
 
+int gg_joinagg_create(gg_engine *e, const gg_scan *outer, const gg_scan *inner, const gg_hashjoin *hj,
+                      const gg_agg *agg, const gg_exprpool *pool, gg_joinagg **out)
+{
+	if (!e || !outer || !inner || !hj || !agg || !pool || !out) return GG_ERR_ARG;
+	return joinagg_create(e, outer, inner, hj, agg, nullptr, 0, pool, out);
+}
+
+int gg_joinrows_create(gg_engine *e, const gg_scan *outer, const gg_scan *inner, const gg_hashjoin *hj,
+                       const int32_t *targets, int ntargets, const gg_exprpool *pool, gg_joinagg **out)
+{
+	if (!e || !outer || !inner || !hj || !targets || !pool || !out) return GG_ERR_ARG;
+	return joinagg_create(e, outer, inner, hj, nullptr, targets, ntargets, pool, out);
+}
+
+/* a right / full join also writes the inner rows no outer row matched (the fill-inner launch after every probe) */
+static bool joinrows_fill_inner(const gg_joinagg *j)
+{
+	return j->jp.jointype == GG_JOIN_RIGHT || j->jp.jointype == GG_JOIN_FULL;
+}
+
+/* Room for `rows` joined rows written by `launches` kernel launches, plus the claim windows' slack: the probe's warps claim
+ * rows `window` at a time (as a sending Motion does, MotionOut.window), and every launch starts with empty windows and marks
+ * what each warp left unused of its last one dead, so each launch leaves at most one window per warp partly unused.  The
+ * window is sized from the rows of one launch, which keeps all tails together below 1/8 of the rows.  Keeps a buffer that is
+ * large enough already. */
+static int joinrows_reserve(gg_joinagg *j, uint64_t rows, uint64_t launches)
+{
+	gg_scanagg *p = j->probe;
+	const uint64_t warps = (uint64_t) p->grid * (uint64_t) (p->cfg.threads / 32 - 1);
+	if (launches < 1) launches = 1;
+	const uint64_t w = rows / launches / (warps * 8);
+	uint32_t window = 0;
+	if (w >= 32) { window = 32; while (window * 2 <= w && window < 1024) window *= 2; }
+	const uint64_t cap = (rows + launches * warps * window + 1) & ~1ull;
+	const uint64_t W = 1 + (uint64_t) j->ntargets;
+	const uint64_t nb = ((cap * W + 8) * 8 + GG_BLCKSZ - 1) / GG_BLCKSZ;      /* + 64 bytes: bulk copies read whole 16 bytes */
+	if (j->rows_buf && j->rows_buf->nblocks < nb) { GG_CUDA(cudaStreamSynchronize(j->eng->stream)); gg_relation_free(j->rows_buf); j->rows_buf = nullptr; }
+	if (!j->rows_buf)
+	{
+		int rc = gg_relation_create(j->eng, nb, &j->rows_buf);
+		if (rc) { j->rows_buf = nullptr; gg_set_error("join output of %llu rows does not fit in device memory", (unsigned long long) cap); return rc; }
+	}
+	MotionOut &mo = p->mo;
+	mo.rows = (unsigned long long *) j->rows_buf->pages;
+	mo.cap = cap;
+	mo.nsegs = 1;
+	mo.rowwords = (int) W;
+	mo.hashtypes = 0;
+	mo.window = window;
+	mo.route = 0; mo.shift = 0;
+	return GG_OK;
+}
+
 /* MultiExecHash: size the table from the inner relation's line pointers (ExecChooseHashTableSize sizes from the
  * planner's row estimate, nodeHash.c:463; the pages give a tight bound for free), then one scan inserts. */
 int gg_joinagg_build(gg_joinagg *j, gg_relation *inner, uint64_t first_block, uint64_t nblocks)
 {
 	if (!j || !inner || nblocks > inner->nblocks || first_block > inner->nblocks - nblocks) return GG_ERR_ARG;
+	if (j->rows_view) { gg_set_error("the joined rows were already handed out: reset before building again"); return GG_ERR_ARG; }
 	if (inner->rowwords != j->jp.build.outer.rowwords) { gg_set_error("inner relation format does not match the plan's tuple descriptor"); return GG_ERR_ARG; }
 	if (inner->rowwords && (first_block != 0 || nblocks != inner->nblocks)) { gg_set_error("datum-row relations are scanned whole"); return GG_ERR_ARG; }
 	gg_engine *e = j->eng;
@@ -242,8 +322,18 @@ int gg_joinagg_build(gg_joinagg *j, gg_relation *inner, uint64_t first_block, ui
 
 int gg_joinagg_probe(gg_joinagg *j, gg_relation *outer, uint64_t first_block, uint64_t nblocks)
 {
-	if (!j) return GG_ERR_ARG;
+	if (!j || !outer) return GG_ERR_ARG;
 	if (j->filled) { gg_set_error("the unmatched inner rows were already emitted: reset before probing again"); return GG_ERR_ARG; }
+	if (j->rows_view) { gg_set_error("the joined rows were already handed out: reset before probing again"); return GG_ERR_ARG; }
+	if (j->ntargets && !j->rows_buf)
+	{
+		/* the output is sized once, from the outer rows (+ the inner rows a right / full join may add); gg_joinagg_rows grows
+		 * it and probes again if the join turns out to produce more */
+		uint64_t nouter = 0;
+		int rc = gg_relation_count_rows(outer, &nouter);
+		if (rc == GG_OK) rc = joinrows_fill_inner(j) ? joinrows_reserve(j, nouter + j->rows_built, 2) : joinrows_reserve(j, nouter, 1);
+		if (rc) return rc;
+	}
 	if (j->lasj_empty) return GG_OK;          /* x NOT IN (.., NULL, ..): no outer row can qualify */
 	return gg_scanagg_run(j->probe, outer, first_block, nblocks);
 }
@@ -251,6 +341,7 @@ int gg_joinagg_probe(gg_joinagg *j, gg_relation *outer, uint64_t first_block, ui
 int gg_joinagg_probe_host(gg_joinagg *j, const void *host_pages, uint64_t nblocks)
 {
 	if (!j) return GG_ERR_ARG;
+	if (j->ntargets) { gg_set_error("a join with a target list probes device-resident relations"); return GG_ERR_UNSUPPORTED; }
 	if (j->filled) { gg_set_error("the unmatched inner rows were already emitted: reset before probing again"); return GG_ERR_ARG; }
 	if (j->lasj_empty) return GG_OK;
 	return gg_scanagg_run_host(j->probe, host_pages, nblocks);
@@ -279,6 +370,7 @@ static int joinagg_fill_inner(gg_joinagg *j)
 int gg_joinagg_fetch(gg_joinagg *j, gg_aggrow *out, int outcap, int *nout, uint64_t *rows_joined)
 {
 	if (!j) return GG_ERR_ARG;
+	if (j->ntargets) { gg_set_error("a join with a target list returns rows (gg_joinagg_rows), not aggregate rows"); return GG_ERR_ARG; }
 	if (j->bj && j->nbatch > 1) return gg_scanagg_fetch(j->bj->probe, out, outcap, nout, nullptr, rows_joined);   /* every batch was filled as it went */
 	int rc = joinagg_fill_inner(j);
 	if (rc) return rc;
@@ -314,6 +406,7 @@ static int joinagg_prepare_batches(gg_joinagg *j)
 	std::vector<int32_t> ov, iv;
 	const int32_t above[] = { j->hj.joinqual };
 	for (int32_t r : above) { collect_vars(pool, r, 0, ov); collect_vars(pool, r, 1, iv); }
+	for (int t = 0; t < j->ntargets; t++) { collect_vars(pool, j->targets[t], 0, ov); collect_vars(pool, j->targets[t], 1, iv); }
 	for (int c = 0; c < j->agg.numCols; c++) { collect_vars(pool, j->agg.grpCol[c], 0, ov); collect_vars(pool, j->agg.grpCol[c], 1, iv); }
 	for (int a = 0; a < j->agg.numAggs; a++) { collect_vars(pool, j->agg.aggs[a].arg, 0, ov); collect_vars(pool, j->agg.aggs[a].arg, 1, iv); }
 	const int nk = j->hj.nkeys;
@@ -367,7 +460,8 @@ static int joinagg_prepare_batches(gg_joinagg *j)
 			a.attnotnull = (x.kind == GG_E_VAR && x.varattno >= 1 && x.varattno <= base.desc.natts) ? base.desc.attrs[x.varattno - 1].attnotnull : 0;
 		}
 	}
-	int rc = gg_joinagg_create(j->eng, &os, &is, &hj2, &j->agg, &bp, &j->bj);
+	/* the targets keep their roots: the Vars under them were renumbered in place */
+	int rc = joinagg_create(j->eng, &os, &is, &hj2, j->ntargets ? nullptr : &j->agg, j->targets, j->ntargets, &bp, &j->bj);
 	if (rc) return rc;
 	/* the inner relation is partitioned by a program that sees it as "the scan": its Vars as varno 0 */
 	j->ipool = new gg_exprpool(pool);
@@ -412,6 +506,8 @@ int gg_joinagg_nbatch(gg_joinagg *j) { return j ? j->nbatch : 0; }
 int gg_joinagg_run(gg_joinagg *j, gg_relation *inner, gg_relation *outer)
 {
 	if (!j || !inner || !outer) return GG_ERR_ARG;
+	/* the rows handed out live in the output buffer this run would rewrite (or reallocate) */
+	if (j->rows_view) { gg_set_error("the joined rows were already handed out: reset before running again"); return GG_ERR_ARG; }
 	gg_engine *e = j->eng;
 	uint64_t nlp = 0;
 	int rc = gg_relation_count_rows(inner, &nlp);
@@ -479,6 +575,10 @@ int gg_joinagg_run(gg_joinagg *j, gg_relation *inner, gg_relation *outer)
 	GG_CUDA(cudaEventElapsedTime(&j->part_ms, j->ev0, j->ev1));
 	rc = gg_scanagg_reset(j->bj->probe);
 	if (rc) return rc;
+	/* every batch appends its rows to the one output of the batch join */
+	if (j->ntargets)
+		rc = joinrows_fill_inner(j) ? joinrows_reserve(j->bj, nouter + nlp, 2 * (uint64_t) nbatch) : joinrows_reserve(j->bj, nouter, (uint64_t) nbatch);
+	if (rc) return rc;
 	j->bj->probe->replay_hook = [j]() { return joinagg_run_batches(j); };
 	return joinagg_run_batches(j);
 }
@@ -488,6 +588,7 @@ int gg_scanagg_groups(gg_scanagg *p, gg_groups **out);
 int gg_joinagg_groups(gg_joinagg *j, gg_groups **out)
 {
 	if (!j) return GG_ERR_ARG;
+	if (j->ntargets) { gg_set_error("a join with a target list returns rows (gg_joinagg_rows), not group records"); return GG_ERR_ARG; }
 	if (!(j->bj && j->nbatch > 1))
 	{
 		int rc = joinagg_fill_inner(j);          /* right / full joins: the unmatched inner rows belong to the result */
@@ -502,6 +603,71 @@ int gg_joinagg_groups(gg_joinagg *j, gg_groups **out)
 	return gg_scanagg_groups(p, out);
 }
 
+/* the probe's status words and row cursor */
+static int joinrows_status(gg_scanagg *p, gg_scanagg::Status *st, unsigned long long *cursor)
+{
+	cudaStream_t s = p->eng->stream;
+	GG_CUDA(cudaMemcpyAsync(st, p->d_status, sizeof *st, cudaMemcpyDeviceToHost, s));
+	GG_CUDA(cudaMemcpyAsync(cursor, p->mo.cursor, sizeof *cursor, cudaMemcpyDeviceToHost, s));
+	GG_CUDA(cudaStreamSynchronize(s));
+	return GG_OK;
+}
+
+int gg_joinagg_rows(gg_joinagg *j, gg_relation **rows, uint64_t *nrows, uint64_t *nlive)
+{
+	if (!j || !rows || !nrows || !nlive) return GG_ERR_ARG;
+	if (!j->ntargets) { gg_set_error("the join has no target list: its matches feed the aggregate above it"); return GG_ERR_ARG; }
+	if (!j->rows_view)
+	{
+		const bool batched = j->bj && j->nbatch > 1;
+		gg_joinagg *r = batched ? j->bj : j;            /* the join whose probe wrote the rows */
+		gg_scanagg *p = r->probe;
+		GG_CUDA(cudaSetDevice(j->eng->device));
+		int rc = batched ? GG_OK : joinagg_fill_inner(j);         /* right / full joins: the unmatched inner rows belong to the result */
+		if (rc) return rc;
+		if (!r->rows_buf) { gg_set_error("no probe has run"); return GG_ERR_ARG; }
+		if (p->build_err)
+		{
+			rc = gg_errflags_to_code(p->build_err);       /* the hash table holds a value the device refused */
+			if (rc) return rc;
+		}
+		gg_scanagg::Status st;
+		unsigned long long cur = 0;
+		rc = joinrows_status(p, &st, &cur);
+		if (rc) return rc;
+		if ((st.err & GGP_EF_TABLE_FULL) && cur > p->mo.cap)
+		{
+			/* The join produced more rows than the output holds.  The cursor counted every row claimed, so one buffer of that
+			 * size, plus the windows' slack of the launches the replay makes (those of the first pass, `fed`), holds them all:
+			 * grow it and probe again against the kept table(s), exactly once. */
+			rc = joinrows_reserve(r, cur, (uint64_t) p->fed.size());
+			if (rc) return rc;
+			if (!batched && p->jt.mark_matched)
+			{
+				/* the replayed fill-inner pass must see only what the replayed probe matches */
+				gg_clear_matched_kernel<<<j->eng->sm_count * 4, 256, 0, j->eng->stream>>>(j->ent, j->slots, p->jt.stride);
+				GG_CUDA(cudaGetLastError());
+				j->eng->launches++;
+			}
+			rc = scanagg_replay(p, MODE_PART, 0);
+			if (rc == GG_OK) rc = joinrows_status(p, &st, &cur);
+			if (rc) return rc;
+			if ((st.err & GGP_EF_TABLE_FULL) && cur > p->mo.cap)
+			{ gg_set_error("join output: %llu rows claimed, capacity %llu after growing", cur, (unsigned long long) p->mo.cap); return GG_ERR_NOMEM; }
+		}
+		rc = gg_errflags_to_code(st.err);
+		if (rc) return rc;
+		j->rows_n = cur < p->mo.cap ? cur : p->mo.cap;
+		j->rows_live = st.counters[1];
+		rc = gg_relation_attach_rows(j->eng, r->rows_buf->pages, j->rows_n, j->ntargets, &j->rows_view);
+		if (rc) { j->rows_view = nullptr; return rc; }
+	}
+	*rows = j->rows_view;
+	*nrows = j->rows_n;
+	*nlive = j->rows_live;
+	return GG_OK;
+}
+
 int gg_joinagg_reset(gg_joinagg *j)
 {
 	if (!j) return GG_ERR_ARG;
@@ -513,6 +679,7 @@ int gg_joinagg_reset(gg_joinagg *j)
 		j->eng->launches++;
 	}
 	j->filled = false;
+	if (j->rows_view) { gg_relation_free(j->rows_view); j->rows_view = nullptr; }
 	if (j->bj) { int rc = gg_joinagg_reset(j->bj); if (rc) return rc; }
 	return gg_scanagg_reset(j->probe);
 }
@@ -539,7 +706,9 @@ void gg_joinagg_free(gg_joinagg *j)
 	if (j->obuf) gg_relation_free(j->obuf);
 	if (j->ibuf) gg_relation_free(j->ibuf);
 	if (j->probe) gg_scanagg_free(j->probe);
-	cudaFree(j->ent); cudaFree(j->d_cnt); cudaFree(j->d_buildcnt);
+	if (j->rows_view) gg_relation_free(j->rows_view);
+	if (j->rows_buf) gg_relation_free(j->rows_buf);
+	cudaFree(j->ent); cudaFree(j->d_cnt); cudaFree(j->d_buildcnt); cudaFree(j->d_rowcur);
 	if (j->ev0) cudaEventDestroy(j->ev0);
 	if (j->ev1) cudaEventDestroy(j->ev1);
 	delete j;

@@ -81,6 +81,7 @@ static inline bool gg_scan_config(gg_launch &c, int mode, bool join, const ggp_p
 	const int V = P.nslots > 0 ? P.nslots : 1;
 	int scr = (P.outer.ncols * 64 + 15) & ~15;                   /* column offsets [ncols][32] u16 */
 	if (mode == GGL_TR || mode == GGL_TRN) scr += V * 33 * 8 + 128 + 128;      /* + transposed values, group ids, null masks */
+	if (mode == GGL_PART) scr += 512;                            /* + the warp's row claim windows (the probe that writes rows) */
 	scr = (scr + 15) & ~15;
 	/* datum-row plans can be fed from column files (gg_scanagg_run_aocs): 32 staged rows per warp at the tail of its scratch */
 	if (P.outer.rowwords) scr += 32 * ((P.outer.rowwords | 1) * 8);

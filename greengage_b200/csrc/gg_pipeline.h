@@ -37,6 +37,8 @@ struct gg_scanagg {
 	int chunks_per_page = 0;        /* 32-row chunks per page of the relation being scanned (0: not sampled yet) */
 	int items_per_page = 0;         /* line pointers of the sampled page */
 	bool is_join = false;           /* probe side of a gg_joinagg: prog = the probe program, jt = the built table */
+	bool join_rows = false;         /* probe of a join with a target list: MODE_PART, every joined row written through `mo` */
+	ggd::MotionOut mo = {};         /* join_rows: the output rows (one destination) and their cursor */
 	ggd::HashAggTable ha = {};           /* MODE_HASH: the group table in HBM */
 	void *ha_mem = nullptr;
 	uint64_t ha_cap = 0;
@@ -77,6 +79,9 @@ struct gg_scanagg {
 int scanagg_finish_create(gg_scanagg *p, gg_scanagg **out);      /* after p->prog / p->aggmap are compiled */
 /* one launch of the pipeline's kernel over device pages (fill_inner: the HJ_FILL_INNER_TUPLES pass of a right/full join) */
 int scanagg_launch(gg_scanagg *p, const uint8_t *dev_pages, uint64_t nblocks, cudaStream_t st, uint64_t nrows = 0, bool fill_inner = false, int32_t aocs_tile_rows = 0);
+/* reset the pipeline and feed its inputs again (through replay_hook when set) on kernel variant `mode` (MODE_HASH: a group
+ * table of ha_cap slots) */
+extern "C" int scanagg_replay(gg_scanagg *p, int mode, uint64_t ha_cap);
 /* gg_motion.cu: the partitioning kernel behind gg_motion_partition, with the routing rule as a parameter (route 0: segments by
  * cdbhash + jump consistent hash; route 1: hash-join batches by the batch bits above `shift`) */
 int gg_partition_rows(gg_engine *e, const gg_scan *scan, const gg_exprpool *pool,
@@ -94,3 +99,4 @@ int gg_scan_kernel(const ggp_program *prog, int mode, int probe_pc, const gg_lau
 __global__ void gg_joinhash_kernel(const __grid_constant__ ggp_program P, const ggd::ScanAggParams prm);
 __global__ void gg_joinbuild_kernel(const __grid_constant__ ggp_program P, const ggd::ScanAggParams prm);
 __global__ void gg_motion_part_kernel(const __grid_constant__ ggp_program P, const ggd::ScanAggParams prm);
+__global__ void gg_joinrows_kernel(const __grid_constant__ ggp_program P, const ggd::ScanAggParams prm);

@@ -245,6 +245,10 @@ int ggp_compile_motion(const gg_scan *scan, const gg_exprpool *pool, const int32
                        char *err, int errlen);
 int ggp_compile_join(const gg_scan *outer, const gg_scan *inner, const gg_hashjoin *hj, const gg_agg *agg,
                      const gg_exprpool *pool, ggp_joinprog *jp, ggp_aggmap *aggmap, char *err, int errlen);
+/* HashJoin with a target list: the same build program; the probe's per-match piece is the join qual FILTER, then GROUP (= claim
+ * an output row) and one OUT per target (1..16, Vars with varno 0 outer / 1 inner) */
+int ggp_compile_joinrows(const gg_scan *outer, const gg_scan *inner, const gg_hashjoin *hj, const int32_t *targets, int ntargets,
+                         const gg_exprpool *pool, ggp_joinprog *jp, char *err, int errlen);
 #endif
 
 #endif /* GG_PROGRAM_H */

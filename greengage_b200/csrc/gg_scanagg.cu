@@ -296,7 +296,7 @@ static const void *const interp_kernels[2][6] = {
 	{ (const void *) gg_scanagg_kernel<MODE_PRIV>, (const void *) gg_scanagg_kernel<MODE_TR>, (const void *) gg_scanagg_kernel<MODE_TRN>,
 	  (const void *) gg_joinbuild_kernel, (const void *) gg_motion_part_kernel, (const void *) gg_hashagg_kernel },
 	{ (const void *) gg_joinprobe_kernel<MODE_PRIV>, (const void *) gg_joinprobe_kernel<MODE_TR>, (const void *) gg_joinprobe_kernel<MODE_TRN>,
-	  nullptr, nullptr, (const void *) gg_joinhash_kernel },
+	  nullptr, (const void *) gg_joinrows_kernel, (const void *) gg_joinhash_kernel },
 };
 
 /* the plan-specialised kernel for a launch shape, or nullptr (why: jmsg) */
@@ -309,7 +309,9 @@ static gg_jit_kernel *scan_jit(const ggp_program *prog, int mode, int probe_pc, 
 int gg_scan_kernel(const ggp_program *prog, int mode, int probe_pc, const gg_launch &c, int device, bool mvcc, const void **fn, gg_jit_kernel **jit)
 {
 	char jmsg[512];
-	gg_jit_kernel *jk = scan_jit(prog, mode, probe_pc, c, device, mvcc, jmsg, sizeof jmsg);
+	gg_jit_kernel *jk = nullptr;
+	if (probe_pc >= 0 && mode == MODE_PART) snprintf(jmsg, sizeof jmsg, "the probe that writes join rows has no specialised kernel");
+	else jk = scan_jit(prog, mode, probe_pc, c, device, mvcc, jmsg, sizeof jmsg);
 	if (jit) *jit = jk;
 	if (!jk && getenv("GGB200_JIT_VERBOSE")) fprintf(stderr, "ggb200: interpreter kernel in use (%s)\n", jmsg);
 	if (!jk && mode != MODE_PRIV && c.threads != 256) { gg_set_error("GGB200_NP_CONFIG needs the run-time specialised kernel: %s", jmsg); return GG_ERR_UNSUPPORTED; }
@@ -391,7 +393,7 @@ int scanagg_launch(gg_scanagg *p, const uint8_t *dev_pages, uint64_t nblocks, cu
 	prm.cnt_off = p->cfg.cnt_off;
 	prm.acc_off = p->cfg.acc_off;
 	prm.jt = p->jt;
-	memset(&prm.mo, 0, sizeof prm.mo);
+	prm.mo = p->mo;
 	prm.nrows = nrows;
 	prm.fill_inner = fill_inner ? 1 : 0;
 	prm.team = p->cfg.team;
@@ -444,7 +446,7 @@ int scanagg_launch(gg_scanagg *p, const uint8_t *dev_pages, uint64_t nblocks, cu
 	p->kev_used++;
 	e->launches++;
 	p->has_state = true;
-	if (p->mode == MODE_HASH) return GG_OK;         /* the group table lives in HBM across launches: nothing to fold */
+	if (p->mode == MODE_HASH || p->mode == MODE_PART) return GG_OK;     /* group table in HBM / rows written: nothing to fold */
 	/* fold the block records (and the previously merged groups) */
 	ggp_acckinds kinds;
 	memcpy(kinds.k, p->prog.acckind, sizeof kinds.k);
@@ -496,7 +498,8 @@ int scanagg_finish_create(gg_scanagg *p, gg_scanagg **out)
 	p->mode = p->prog.nullable ? MODE_TRN : MODE_TR;
 	if (p->prog.priv_ok) p->mode = MODE_PRIV;
 	const char *force = getenv("GGB200_SCAN_MODE");           /* experiments: 0 PRIV, 1 TR, 2 TRN, 5 HASH */
-	if (force && atoi(force) == MODE_HASH) p->mode = MODE_HASH;
+	if (p->join_rows) p->mode = MODE_PART;
+	else if (force && atoi(force) == MODE_HASH) p->mode = MODE_HASH;
 	else if (force && !p->is_join)
 	{ int m = atoi(force); if (m == MODE_PRIV && !p->prog.priv_ok) m = MODE_TR; if (p->prog.nullable) m = MODE_TRN; p->mode = m; }
 	rc = scanagg_configure(p);
@@ -557,6 +560,7 @@ int gg_scanagg_reset(gg_scanagg *p)
 	p->fed.clear();
 	GG_CUDA(cudaMemsetAsync(p->merged, 0, sizeof(ggp_grec) * GG_MERGE_CAP, st));
 	GG_CUDA(cudaMemsetAsync(p->d_status, 0, sizeof(gg_scanagg::Status), st));
+	if (p->mo.cursor) GG_CUDA(cudaMemsetAsync(p->mo.cursor, 0, sizeof(unsigned long long), st));
 	p->has_state = false;
 	p->kev_used = 0;
 	if (p->mode == MODE_HASH)
@@ -877,7 +881,7 @@ static int records_to_rows(const gg_agg *agg, const ggp_aggmap *aggmap, const ui
 /* Run the fed inputs again on kernel variant `mode` (MODE_HASH: into a group table of `ha_cap` slots): reconfigure, reset, and
  * feed everything again — through the batched join's replay_hook when there is one — like the reference's hybrid hash
  * aggregate re-reading spilled input (execHHashagg.c:1093). */
-static int scanagg_replay(gg_scanagg *p, int mode, uint64_t ha_cap)
+int scanagg_replay(gg_scanagg *p, int mode, uint64_t ha_cap)
 {
 	gg_engine *e = p->eng;
 	std::vector<gg_scanagg::Fed> replay = p->fed;

@@ -24,7 +24,8 @@
  *     MODE_BUILD     Hash node: join keys + payload columns into the join hash table
  *     JOIN = true    (with PRIV / TR / TRN / HASH) the probe side: every outer row probes the table and each match
  *                    runs the per-match piece of the program; also the fill-inner pass of right / full joins
- *     MODE_PART      sending Motion: cdbhash + jump consistent hash, rows packed per destination
+ *     MODE_PART      sending Motion: cdbhash + jump consistent hash, rows packed per destination; with JOIN = true the
+ *                    probe of a join with a target list: every joined row written as a datum row (JoinRowSink)
  *   epilogue         PRIV / TR: threads -> one record per group and block -> global; a single-block merge kernel
  *                    folds records with equal keys.  Every reduction tree is fixed => sums are bit-identical run to
  *                    run.
@@ -570,6 +571,31 @@ struct PartSink {
 		else row[1 + slot] = (unsigned long long) __double_as_longlong(v);
 	}
 };
+/* the probe of a join with a target list (gg_joinrows_create): PartSink's row claim and output into one destination (claim
+ * windows, dead marking at the end), plus what the probe loop asks of a join sink.  KEY = join key (first program piece);
+ * in the per-match piece FILTER = the join qual, GROUP = claim a row, OUT = target column.  The row's NULL mask follows the
+ * null-extended side: its columns evaluate to NULL. */
+struct JoinRowSink : PartSink {
+	uint32_t keytypes;
+	uint64_t k0, k1;
+	uint32_t knull;
+	bool jq, nullext, suppress;
+	__device__ __forceinline__ void begin_row() { PartSink::begin_row(); k0 = k1 = 0; knull = 0; }
+	__device__ __forceinline__ bool filter_match(bool pass)
+	{
+		if (nullext) return true;
+		jq = pass;
+		return pass && !suppress;
+	}
+	__device__ __forceinline__ void key(int kc, uint64_t v, bool isnull)
+	{
+		if (isnull) { knull |= 1u << kc; return; }
+		v = group_key(v, (int) ((keytypes >> (2 * kc)) & 3));
+		if (kc == 0) k0 = v; else k1 = v;
+	}
+	/* ANTI probing a match: the join qual was evaluated, no row is written */
+	__device__ __forceinline__ bool group(bool live) { return PartSink::group(live && !suppress); }
+};
 /* general HashAggregate: KEY = grouping key, GROUP = find or insert the group's slot, OUT = advance one transition value */
 struct HashSink {
 	HashAggTable ha;
@@ -677,7 +703,8 @@ struct HashSink {
 };
 template <int MODE, bool JOIN> struct SinkSel { typedef RowSink<MODE, JOIN> type; };
 template <bool JOIN> struct SinkSel<MODE_HASH, JOIN> { typedef HashSink type; };
-template <bool JOIN> struct SinkSel<MODE_PART, JOIN> { typedef PartSink type; };
+template <> struct SinkSel<MODE_PART, false> { typedef PartSink type; };
+template <> struct SinkSel<MODE_PART, true> { typedef JoinRowSink type; };
 template <bool JOIN> struct SinkSel<MODE_BUILD, JOIN> { typedef BuildSink type; };
 
 /* Line pointer -> tuple: ItemId decode, the sanity rules of PageAddItem, the visibility fast path, header checks.
@@ -1003,6 +1030,7 @@ __device__ __forceinline__ void scanagg_body(const ggp_program &P, const ScanAgg
 			sink.win = sv;                       /* the per-warp scratch behind the column offsets */
 			sts64(sv + (uint32_t) lane * 16, 0); sts64(sv + (uint32_t) lane * 16 + 8, 0);
 			__syncwarp();
+			if constexpr (JOIN) { sink.keytypes = PL::keytypes(P); sink.jq = false; sink.nullext = false; sink.suppress = false; }
 		}
 		else if constexpr (MODE == MODE_HASH)
 		{

@@ -238,6 +238,38 @@ class JoinAgg:
             self.h = C.c_void_p()
 
 
+class JoinRows(JoinAgg):
+    """HashJoin with a target list (gg_joinrows_create): build / probe / run / reset / stats as JoinAgg; rows() instead of
+    fetch()."""
+
+    def __init__(self, eng, outer, inner, hj, targets, pool):
+        self.eng = eng
+        self.h = C.c_void_p()
+        self.ncols = len(targets)
+        t = (C.c_int32 * max(1, len(targets)))(*targets)
+        check(dev_lib().gg_joinrows_create(eng.h, C.byref(outer), C.byref(inner), C.byref(hj), t, len(targets), C.byref(pool),
+                                           C.byref(self.h)))
+
+    def rows_raw(self):
+        """(the output relation handle, slots, rows joined): gg_joinagg_rows"""
+        rel, n, live = C.c_void_p(), C.c_uint64(0), C.c_uint64(0)
+        check(dev_lib().gg_joinagg_rows(self.h, C.byref(rel), C.byref(n), C.byref(live)))
+        return rel, n.value, live.value
+
+    def rows(self):
+        """the joined rows on the host, dead slots dropped: (values int64 [n][ncols], isnull bool [n][ncols], rows joined)"""
+        rel, n, live = self.rows_raw()
+        W = 1 + self.ncols
+        nb = (n * W * 8 + capi.GG_BLCKSZ - 1) // capi.GG_BLCKSZ
+        buf = np.zeros(nb * capi.GG_BLCKSZ // 8, dtype=np.uint64)
+        if nb:
+            check(dev_lib().gg_relation_read(rel, 0, buf.ctypes.data, nb))
+        r = buf[:n * W].reshape(n, W)
+        r = r[(r[:, 0] & np.uint64(1 << 63)) == 0]
+        nulls = ((r[:, :1] >> np.arange(self.ncols, dtype=np.uint64)) & np.uint64(1)).astype(bool)
+        return np.ascontiguousarray(r[:, 1:]).view(np.int64), nulls, live
+
+
 def sort_rows(eng, keys, rows, nulls=None):
     """Sort n x ncols int64 Datum rows (host numpy) on the device; returns the sorted permutation (uint64)."""
     import numpy as np

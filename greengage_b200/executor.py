@@ -40,7 +40,7 @@ class GgHash(C.Structure):
 
 
 class GgHashJoin(C.Structure):
-    _fields_ = [("plan", GgPlan), ("hj", capi.gg_hashjoin)]
+    _fields_ = [("plan", GgPlan), ("hj", capi.gg_hashjoin), ("numTargets", C.c_int32), ("targets", C.c_int32 * GG_MAX_OUTCOLS)]
 
 
 class GgSort(C.Structure):
@@ -168,10 +168,15 @@ class PlanBuilder:
         n.plan.type, n.plan.qual, n.plan.lefttree = T_Hash, -1, _as_plan(child)
         return n
 
-    def hashjoin(self, outer, hashnode, hj):
+    def hashjoin(self, outer, hashnode, hj, targets=()):
+        """targets: expression roots the join projects (varno 0 outer, 1 inner; its rows stay on the device for the node
+        above); () = fused with the Agg above"""
         n = self._keep(GgHashJoin())
         n.plan.type, n.plan.qual, n.plan.lefttree, n.plan.righttree = T_HashJoin, -1, _as_plan(outer), _as_plan(hashnode)
         C.memmove(C.byref(n.hj), C.byref(hj), C.sizeof(capi.gg_hashjoin))
+        n.numTargets = len(targets)
+        for i, t in enumerate(targets):
+            n.targets[i] = t
         return n
 
     def sort(self, child, keys):

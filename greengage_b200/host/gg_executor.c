@@ -13,6 +13,8 @@
  *                      (gg_ic_motion_groups, gg_groups_final); the node at the top fetches once
  *     scanned rows     as datum rows (GG_FMT_DATUMROWS): SeqScan with a target list -> Redistribute Motion ->
  *                      Hash / HashJoin / Agg scan them with the same kernels (gg_motion_partition, gg_ic_exchange_rows)
+ *     joined rows      as datum rows: a HashJoin with a target list writes them (gg_joinrows_create) for another HashJoin,
+ *                      a Sort / Limit, a Motion or the caller
  * Host arrays of Datums appear only where a node has to hand tuples to its caller, or on the generic path (Sort, a
  * Motion over a transport callback).
  */
@@ -26,7 +28,7 @@
 int32_t gg_cdbhash_route(const int32_t *typids, const int64_t *vals, const int32_t *lens, const int32_t *isnull,
                          int nkeys, int nsegs);      /* gg_motion_host.c */
 
-enum { K_SCANAGG = 1, K_JOINAGG, K_AGGFINAL, K_SORT, K_MOTION, K_SCANROWS, K_HASH, K_LIMIT };
+enum { K_SCANAGG = 1, K_JOINAGG, K_AGGFINAL, K_SORT, K_MOTION, K_SCANROWS, K_HASH, K_LIMIT, K_JOINROWS };
 
 #define GG_NO_BOUND UINT64_MAX
 
@@ -35,6 +37,9 @@ enum { K_SCANAGG = 1, K_JOINAGG, K_AGGFINAL, K_SORT, K_MOTION, K_SCANROWS, K_HAS
  * keeps its CPU nodes for that subtree; no other sort takes their place. */
 #pragma weak gg_sort_rows_bounded
 #pragma weak gg_sort_datumrows_bounded
+/* the same for the join that writes its rows: without them a HashJoin with a target list is refused (GG_ERR_UNSUPPORTED) */
+#pragma weak gg_joinrows_create
+#pragma weak gg_joinagg_rows
 
 struct GgPlanState {
 	int kind;
@@ -42,6 +47,8 @@ struct GgPlanState {
 	GgEState *estate;
 	struct GgPlanState *child;          /* Sort / Motion / final Agg / Agg over rows: the pipeline below */
 	struct GgPlanState *inner;          /* join: the rows node under the Hash (NULL: the inner SeqScan is fused) */
+	int table_kept;                     /* K_JOINROWS: the hash table of one batch is built and kept for a rescan (never with a
+	                                     * Motion on the inner side: every segment re-runs that exchange alike) */
 	/* device pipelines */
 	gg_scanagg *sa;
 	gg_joinagg *ja;
@@ -51,7 +58,8 @@ struct GgPlanState {
 	gg_agg agg;
 	/* device-resident results */
 	gg_groups *groups;                  /* aggregate rows */
-	gg_relation *rows_rel;              /* datum rows (K_SCANROWS, K_MOTION over a scan): wraps rows_recv / rows_send */
+	gg_relation *rows_rel;              /* datum rows (K_SCANROWS, K_MOTION over a scan): wraps rows_recv / rows_send; K_JOINROWS:
+	                                     * wraps the join's output */
 	gg_relation *rows_send, *rows_recv; /* raw device buffers (gg_relation_create) */
 	uint64_t rows_cap;                  /* rows the send buffer holds over all destinations */
 	uint64_t rows_n;
@@ -115,6 +123,7 @@ const char *GgExecNodeKind(GgPlanState *s)
 		case K_SCANROWS: return "scanrows";
 		case K_HASH: return "hash";
 		case K_LIMIT: return "limit";
+		case K_JOINROWS: return "joinrows";
 	}
 	return "";
 }
@@ -327,11 +336,13 @@ GgPlanState *GgExecInitNode(GgPlan *node, GgEState *estate, int eflags)
 
 static int multi_segment(const GgEState *es) { return es->nsegs > 1; }
 
-/* a node that delivers device-resident datum rows: a SeqScan with a target list, or a Motion over one */
+/* a node that delivers device-resident datum rows: a SeqScan with a target list, a Motion over one, or a HashJoin with a
+ * target list */
 static int yields_rows(const GgPlan *p)
 {
 	if (!p) return 0;
 	if (p->type == T_GgSeqScan) return ((const GgSeqScan *) p)->numTargets > 0;
+	if (p->type == T_GgHashJoin) return ((const GgHashJoin *) p)->numTargets > 0;
 	if (p->type == T_GgMotion) return p->lefttree && p->lefttree->type == T_GgSeqScan && ((const GgSeqScan *) p->lefttree)->numTargets > 0;
 	return 0;
 }
@@ -417,6 +428,60 @@ static int init_rows_node(GgPlan *node, GgEState *estate, GgPlanState *s)
 	return 0;
 }
 
+/* a HashJoin pipeline: fused with the Agg above it (agg != NULL, K_JOINAGG), or writing the rows of its target list (K_JOINROWS) */
+static int init_join(GgPlanState *s, GgPlan *node, const gg_agg *agg, int eflags, int depth)
+{
+	GgEState *estate = s->estate;
+	GgHashJoin *hj = (GgHashJoin *) node;
+	GgPlan *outer = node->lefttree, *hash = node->righttree, *inner = hash ? hash->lefttree : NULL;
+	gg_scan oscan, iscan;
+	int rc, i;
+	if (!agg && (!gg_joinrows_create || !gg_joinagg_rows))
+	{ exec_fail(GG_ERR_UNSUPPORTED, "HashJoin with a target list: the device library has no join that writes its rows"); return -1; }
+	if (!agg && (hj->numTargets > GG_MAX_OUTCOLS || hj->numTargets > 16))
+	{ exec_fail(GG_ERR_UNSUPPORTED, "HashJoin projecting %d columns (1..16 travel as datum rows)", hj->numTargets); return -1; }
+	if (!hash || hash->type != T_GgHash || !is_pipeline_input(outer) || !is_pipeline_input(inner))
+	{
+		exec_fail(GG_ERR_UNSUPPORTED, "HashJoin: both inputs must be a SeqScan or a Redistribute Motion over one (Hash on the inner side)");
+		return -1;
+	}
+	s->kind = agg ? K_JOINAGG : K_JOINROWS;
+	if (init_input(s, outer, eflags, depth + 1, &oscan, &s->child, &s->rel)) return -1;
+	if (!s->child && !s->rel) { exec_fail(GG_ERR_UNSUPPORTED, "HashJoin: the outer relation must be resident on the device"); return -1; }
+	if (init_input(s, inner, eflags, depth + 2, &iscan, &s->inner, &s->inner_rel)) return -1;
+	if (!s->inner && !s->inner_rel) { exec_fail(GG_ERR_UNSUPPORTED, "HashJoin: the inner relation must be resident on the device"); return -1; }
+	if (agg)
+	{
+		rc = gg_joinagg_create(estate->engine, &oscan, &iscan, &hj->hj, agg, estate->pool, &s->ja);
+		if (rc != GG_OK) { exec_fail(rc, "Agg <- HashJoin: %s", gg_last_error()); return -1; }
+		s->dev_groups = 1;
+		return 0;
+	}
+	rc = gg_joinrows_create(estate->engine, &oscan, &iscan, &hj->hj, hj->targets, hj->numTargets, estate->pool, &s->ja);
+	if (rc != GG_OK) { exec_fail(rc, "HashJoin: %s", gg_last_error()); return -1; }
+	/* the rows' descriptor: a column of the side a join null-extends is nullable; a plain Var of a NOT NULL column of the other
+	 * side stays NOT NULL, as a scan's projection keeps it */
+	s->rows_ncols = hj->numTargets;
+	s->rows_nsegs = 1;
+	s->ncols = hj->numTargets;
+	memset(&s->rows_desc, 0, sizeof s->rows_desc);
+	s->rows_desc.natts = hj->numTargets;
+	s->rows_desc.format = GG_FMT_DATUMROWS;
+	for (i = 0; i < hj->numTargets; i++)
+	{
+		const gg_expr *e = &estate->pool->nodes[hj->targets[i]];          /* checked by gg_joinrows_create */
+		const int jt = hj->hj.jointype;
+		const int nullext = e->varno == 0 ? (jt == GG_JOIN_RIGHT || jt == GG_JOIN_FULL) : (jt == GG_JOIN_LEFT || jt == GG_JOIN_FULL);
+		const gg_tupdesc *d = e->varno == 0 ? &oscan.desc : &iscan.desc;
+		gg_attr *a = &s->rows_desc.attrs[i];
+		s->rows_targets[i] = hj->targets[i];
+		s->typid[i] = e->rettype;
+		a->atttypid = e->rettype; a->atttypmod = -1; a->attlen = 8; a->attalign = 'd'; a->attbyval = 1;
+		a->attnotnull = (e->kind == 1 /* GG_E_VAR */ && !nullext && e->varattno >= 1 && e->varattno <= d->natts) ? d->attrs[e->varattno - 1].attnotnull : 0;
+	}
+	return 0;
+}
+
 static GgPlanState *init_node(GgPlan *node, GgEState *estate, int eflags, int depth)
 {
 	GgPlanState *s;
@@ -428,7 +493,7 @@ static GgPlanState *init_node(GgPlan *node, GgEState *estate, int eflags, int de
 	s->plan = node; s->estate = estate;
 	if (yields_rows(node))
 	{
-		if (init_rows_node(node, estate, s)) goto fail;
+		if (node->type == T_GgHashJoin ? init_join(s, node, NULL, eflags, depth) : init_rows_node(node, estate, s)) goto fail;
 		return s;
 	}
 	switch (node->type)
@@ -459,6 +524,12 @@ static GgPlanState *init_node(GgPlan *node, GgEState *estate, int eflags, int de
 				}
 				return s;
 			}
+			/* a HashJoin directly below stays fused with this Agg, whether it has a target list or not */
+			if (below && below->type == T_GgHashJoin)
+			{
+				if (init_join(s, below, &an->agg, eflags, depth)) goto fail;
+				return s;
+			}
 			if (is_pipeline_input(below))
 			{
 				gg_scan scan;
@@ -466,26 +537,6 @@ static GgPlanState *init_node(GgPlan *node, GgEState *estate, int eflags, int de
 				if (init_input(s, below, eflags, depth + 1, &scan, &s->child, &s->rel)) goto fail;
 				rc = gg_scanagg_create(estate->engine, &scan, &an->agg, estate->pool, &s->sa);
 				if (rc != GG_OK) { exec_fail(rc, "Agg <- SeqScan: %s", gg_last_error()); goto fail; }
-				s->dev_groups = 1;
-				return s;
-			}
-			if (below && below->type == T_GgHashJoin)
-			{
-				GgHashJoin *hj = (GgHashJoin *) below;
-				GgPlan *outer = below->lefttree, *hash = below->righttree, *inner = hash ? hash->lefttree : NULL;
-				gg_scan oscan, iscan;
-				if (!hash || hash->type != T_GgHash || !is_pipeline_input(outer) || !is_pipeline_input(inner))
-				{
-					exec_fail(GG_ERR_UNSUPPORTED, "HashJoin: both inputs must be a SeqScan or a Redistribute Motion over one (Hash on the inner side)");
-					goto fail;
-				}
-				s->kind = K_JOINAGG;
-				if (init_input(s, outer, eflags, depth + 1, &oscan, &s->child, &s->rel)) goto fail;
-				if (!s->child && !s->rel) { exec_fail(GG_ERR_UNSUPPORTED, "HashJoin: the outer relation must be resident on the device"); goto fail; }
-				if (init_input(s, inner, eflags, depth + 2, &iscan, &s->inner, &s->inner_rel)) goto fail;
-				if (!s->inner && !s->inner_rel) { exec_fail(GG_ERR_UNSUPPORTED, "HashJoin: the inner relation must be resident on the device"); goto fail; }
-				rc = gg_joinagg_create(estate->engine, &oscan, &iscan, &hj->hj, &an->agg, estate->pool, &s->ja);
-				if (rc != GG_OK) { exec_fail(rc, "Agg <- HashJoin: %s", gg_last_error()); goto fail; }
 				s->dev_groups = 1;
 				return s;
 			}
@@ -536,7 +587,7 @@ static GgPlanState *init_node(GgPlan *node, GgEState *estate, int eflags, int de
 			exec_fail(GG_ERR_UNSUPPORTED, "a SeqScan without a target list is only accelerated underneath an Agg or a HashJoin");
 			goto fail;
 		case T_GgHashJoin:
-			/* a join that has to return its rows to a CPU parent: not materialised on the device */
+			/* no target list: nothing says which columns its rows would have (one with a target list yields rows, above) */
 			exec_fail(GG_ERR_UNSUPPORTED, "a HashJoin is only accelerated underneath an Agg (the join is never materialised)");
 			goto fail;
 		case T_GgHash:
@@ -833,6 +884,7 @@ static int run_rows_node(GgPlanState *s)
 /* the device buffer that holds a rows node's datum rows */
 static gg_relation *rows_buffer(const GgPlanState *s)
 {
+	if (s->kind == K_JOINROWS) return s->rows_rel;        /* the join's own output buffer */
 	return s->rows_recv && s->rows_nsegs > 1 ? s->rows_recv : s->rows_send;
 }
 
@@ -1020,25 +1072,54 @@ static int motion_host_path(GgPlanState *s, int child_failed)
 	return 0;
 }
 
-/* Agg <- SeqScan or Agg <- HashJoin: one scan / join pipeline */
+/* a Motion in this subtree: rows cross segments there, so every segment has to run it whenever any does */
+static int has_motion(const GgPlanState *s)
+{
+	return s && (s->kind == K_MOTION || has_motion(s->child) || has_motion(s->inner));
+}
+
+/* Agg <- SeqScan, Agg <- HashJoin, or a HashJoin writing its rows: one scan / join pipeline */
 static int run_agg_pipeline(GgPlanState *s)
 {
 	GgEState *es = s->estate;
 	int rc;
 	drop_device_results(s);
 	if (run_child(s)) return -1;
-	if (s->inner && !s->inner->done && run_node(s->inner)) return -1;
-	if (s->kind == K_SCANAGG)
+	if (s->kind == K_JOINROWS && s->table_kept)
 	{
-		if (s->child) rc = gg_scanagg_run(s->sa, s->child->rows_rel, 0, gg_relation_nblocks(s->child->rows_rel));
-		else if (s->rel) rc = gg_scanagg_run(s->sa, s->rel, 0, gg_relation_nblocks(s->rel));
-		else rc = gg_scanagg_run_host(s->sa, s->host_pages, s->host_nblocks);
+		/* ExecReScanHashJoin (nodeHashjoin.c:1015-1050): the table of the unchanged inner side is kept, only the outer side is
+		 * probed again */
+		gg_relation *outer = s->child ? s->child->rows_rel : s->rel;
+		rc = gg_joinagg_probe(s->ja, outer, 0, gg_relation_nblocks(outer));
 	}
 	else
 	{
-		/* MultiExecHash + the probe loop; in batches when the table would not fit the operator's memory */
-		rc = gg_joinagg_set_work_mem(s->ja, es->es_operator_mem);
-		if (rc == GG_OK) rc = gg_joinagg_run(s->ja, s->inner ? s->inner->rows_rel : s->inner_rel, s->child ? s->child->rows_rel : s->rel);
+		if (s->inner && !s->inner->done && run_node(s->inner)) return -1;
+		if (s->kind == K_SCANAGG)
+		{
+			if (s->child) rc = gg_scanagg_run(s->sa, s->child->rows_rel, 0, gg_relation_nblocks(s->child->rows_rel));
+			else if (s->rel) rc = gg_scanagg_run(s->sa, s->rel, 0, gg_relation_nblocks(s->rel));
+			else rc = gg_scanagg_run_host(s->sa, s->host_pages, s->host_nblocks);
+		}
+		else
+		{
+			/* MultiExecHash + the probe loop; in batches when the table would not fit the operator's memory */
+			rc = gg_joinagg_set_work_mem(s->ja, es->es_operator_mem);
+			if (rc == GG_OK) rc = gg_joinagg_run(s->ja, s->inner ? s->inner->rows_rel : s->inner_rel, s->child ? s->child->rows_rel : s->rel);
+		}
+	}
+	if (rc == GG_OK && s->kind == K_JOINROWS)
+	{
+		/* the joined rows stay on the device for the node above (or come to the host once, at the top) */
+		gg_relation *out;
+		uint64_t live;
+		rc = gg_joinagg_rows(s->ja, &out, &s->rows_n, &live);
+		if (rc == GG_OK) rc = gg_relation_attach_rows(es->engine, gg_relation_device_ptr(out), s->rows_n, s->rows_ncols, &s->rows_rel);
+		if (rc != GG_OK) { s->rows_rel = NULL; exec_fail(rc, "%s", gg_last_error()); return -1; }
+		/* whether a segment batched depends on its own inner rows; a Motion below the Hash is a plan property, the same on
+		 * every segment, so a rescan re-runs that exchange everywhere or nowhere */
+		s->table_kept = gg_joinagg_nbatch(s->ja) == 1 && !has_motion(s->inner);
+		return 0;
 	}
 	if (rc != GG_OK) { exec_fail(rc, "%s", gg_last_error()); return -1; }
 	if (s->lazy_fetch && !es->motion_on_host && pipeline_groups(s) == GG_OK)
@@ -1311,7 +1392,7 @@ static int run_node(GgPlanState *s)
 	switch (s->kind)
 	{
 		case K_SCANROWS: rc = run_rows_node(s); break;
-		case K_SCANAGG: case K_JOINAGG: rc = run_agg_pipeline(s); break;
+		case K_SCANAGG: case K_JOINAGG: case K_JOINROWS: rc = run_agg_pipeline(s); break;
 		case K_AGGFINAL: rc = run_final_agg(s); break;
 		case K_SORT: rc = run_sort(s); break;
 		case K_MOTION: rc = run_motion(s); break;
@@ -1398,8 +1479,8 @@ int GgExecNodeInstrumentation(GgPlanState *s, GgInstrumentation *out)
 	out->ntuples = s->instr_ntuples;
 	out->nloops = s->instr_nloops;
 	out->sort_runs = s->kind == K_SORT ? s->sort_runs : 0;
-	if (s->kind == K_JOINAGG && s->ja) out->hash_batches = gg_joinagg_nbatch(s->ja);
-	if ((s->kind == K_SCANAGG && s->sa) || (s->kind == K_JOINAGG && s->ja))
+	if ((s->kind == K_JOINAGG || s->kind == K_JOINROWS) && s->ja) out->hash_batches = gg_joinagg_nbatch(s->ja);
+	if ((s->kind == K_SCANAGG && s->sa) || ((s->kind == K_JOINAGG || s->kind == K_JOINROWS) && s->ja))
 		if (GgExecPipelineKernelMs(s, &ms, &launches, &variant, &bms) == GG_OK) out->kernel_ms = ms + bms;
 	return GG_OK;
 }

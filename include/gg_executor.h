@@ -14,6 +14,7 @@
  * What ExecInitNode does differently from the reference: it FUSES the slice into device pipelines
  *     Agg <- SeqScan                         one scan+aggregate kernel      (gg_scanagg_*)
  *     Agg <- HashJoin(SeqScan, Hash(SeqScan)) build kernel + probe kernel   (gg_joinagg_*)
+ *     HashJoin with a target list             build kernel + row-writing probe: datum rows (gg_joinrows_create)
  *     Sort <- any of the above                device radix sort             (gg_sort_rows)
  *     Motion <- any of the above              rows handed to the transport  (GgMotionTransport)
  * and returns NULL with GgExecLastError() set when a node or a shape is outside the accelerated subset, so the
@@ -78,8 +79,14 @@ typedef struct GgHash {
 } GgHash;
 
 typedef struct GgHashJoin {
-	GgPlan plan;                    /* lefttree: outer SeqScan; righttree: Hash */
+	GgPlan plan;                    /* lefttree: outer input; righttree: Hash over the inner input */
 	gg_hashjoin hj;
+	/* plan.targetlist: the expressions the join projects, roots in the pool, Vars with varno 0 = outer, 1 = inner (1..16).
+	 * 0 = the Agg directly above reads the joined columns itself (fused, no row is written; refused anywhere else).  > 0: the
+	 * join writes device-resident datum rows of these columns for the node above — another HashJoin, a Sort, a Limit, a
+	 * Motion or the caller.  A join directly under an Agg stays fused whether it has targets or not. */
+	int32_t numTargets;
+	int32_t targets[GG_MAX_OUTCOLS];
 } GgHashJoin;
 
 typedef struct GgSort {
@@ -178,7 +185,8 @@ int  GgExecReScan(GgPlanState *node);
 void GgExecSquelchNode(GgPlanState *node);
 const char *GgExecLastError(void);
 int  GgExecLastErrorCode(void);                /* GG_ERR_* of the failure, GG_OK if none */
-/* introspection: which device pipeline a state node was fused into ("scanagg", "joinagg", "sort", "motion", "limit", ...) */
+/* introspection: which device pipeline a state node was fused into ("scanagg", "joinagg", "joinrows", "sort", "motion",
+ * "limit", ...) */
 const char *GgExecNodeKind(GgPlanState *node);
 /* where a node that has run keeps its result: "device-groups" (aggregate rows as group records), "device-rows" (datum rows)
  * or "host" (Datum arrays); "" before it has run */
@@ -209,9 +217,10 @@ GgPlanState *GgExecInnerPlanState(GgPlanState *node);
  * at link time instead of going through ExecProcNode's switch.  Each checks the node tag and delegates to the
  * functions above; the state they return is the state of the fused pipeline rooted at that node.
  *     nodeAgg.h:22-25,231   nodeSort.h:19-25   nodeMotion.h:20-27   nodeHashjoin.h:20-28   nodeSeqscan.h:19-24
- * A HashJoin or SeqScan is only accelerated underneath an Agg (the join is never materialised), so GgExecInitHashJoin /
- * GgExecInitSeqScan on a bare node return NULL with GG_ERR_UNSUPPORTED, and the Hash node has no state of its own
- * (MultiExecHash is the build kernel the Agg's pipeline launches). */
+ * A HashJoin or SeqScan without a target list is only accelerated underneath an Agg (its rows are never written), so
+ * GgExecInitHashJoin / GgExecInitSeqScan on such a bare node return NULL with GG_ERR_UNSUPPORTED; with a target list they
+ * produce device-resident rows.  The Hash node has no state of its own (MultiExecHash is the build kernel the join's
+ * pipeline launches). */
 GgPlanState *GgExecInitAgg(GgAgg *node, GgEState *estate, int eflags);
 GgTupleTableSlot *GgExecAgg(GgPlanState *node);
 void GgExecEndAgg(GgPlanState *node);

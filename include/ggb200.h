@@ -156,6 +156,19 @@ int  gg_joinagg_reset(gg_joinagg *p);      /* ExecReScanHashJoin with the hash t
 int  gg_joinagg_stats(gg_joinagg *p, uint64_t *rows_built, uint64_t *table_bytes, float *build_ms, float *probe_ms);
 int  gg_joinagg_variant(gg_joinagg *p);       /* kernel variant of the probe side, as gg_scanagg_variant */
 void gg_joinagg_free(gg_joinagg *p);
+/* HashJoin with a target list (ExecHashJoin -> ExecProject, nodeHashjoin.c:78-509): the same pipeline — build, table sizing,
+ * batches, the fill-inner pass of right / full joins, reset, stats, set_work_mem and free are gg_joinagg_*'s — whose probe
+ * writes every joined row as a datum row instead of feeding an aggregate.  targets: 1..16 expression roots in the pool, Vars
+ * with varno 0 = outer, 1 = inner (outer only for SEMI / ANTI / LASJ_NOTIN); numeric targets are refused (GG_ERR_UNSUPPORTED).
+ * The output is sized from the outer rows (+ the inner rows of a right / full join); a join that produces more is probed
+ * once more against the kept table, into a buffer as large as the first probe found it needs. */
+int  gg_joinrows_create(gg_engine *e, const gg_scan *outer, const gg_scan *inner, const gg_hashjoin *hj,
+                        const int32_t *targets, int ntargets, const gg_exprpool *pool, gg_joinagg **out);
+/* after gg_joinagg_run (or build + probe): the joined rows, GG_FMT_DATUMROWS of ntargets columns with the NULL mask of the
+ * null-extended side set; *nrows slots of which some may be dead (GG_DATUMROW_DEAD); *nlive = rows joined.  The relation is
+ * a view owned by the join, valid until gg_joinagg_reset / gg_joinagg_free; building, probing or running again needs a reset
+ * first. */
+int  gg_joinagg_rows(gg_joinagg *p, gg_relation **rows, uint64_t *nrows, uint64_t *nlive);
 
 /* ---- Append-only column-oriented (AOCS) relations ----
  * Decode the projected columns of a segment file, resident in device memory together with the loader's block directories
