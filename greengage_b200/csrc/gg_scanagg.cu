@@ -439,6 +439,9 @@ int scanagg_launch(gg_scanagg *p, const uint8_t *dev_pages, uint64_t nblocks, cu
 		}
 		fn = (const void *) p->jit_snap->kernel;
 	}
+	/* the interpreter kernels are shared by every pipeline, and configuring one sets their shared-memory limit to its own size:
+	 * a pipeline configured later with less (the upper of two joins that write rows) would make this launch fail */
+	GG_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) p->cfg.smem));
 	void *args[] = { (void *) &p->prog, (void *) &prm };
 	GG_CUDA(cudaLaunchKernel(fn, dim3(p->grid), dim3(p->cfg.threads), args, p->cfg.smem, st));
 	GG_CUDA(cudaGetLastError());

@@ -202,6 +202,40 @@ def _check_exact(fn, partial, j, x, e, ctx):
         assert err <= bound, ("avg outside its bound", x, float(s / e.n), float(err), float(bound)) + ctx
 
 
+class _Record:
+    __slots__ = ("n", "flags", "lowbit", "lowbit_sq", "s", "a", "q")
+
+
+def exact_record(values):
+    """What the oracle's exact mode records (po.Exact) for the float8 inputs `values` of one aggregate in one group (NULLs
+    left out), computed here with Fraction: for holding a float8 SUM/AVG computed elsewhere to the same rule"""
+    import math
+    r = _Record()
+    r.n, r.flags, r.lowbit, r.lowbit_sq, r.s, r.a, r.q = len(values), 0, None, None, 0, 0, 0
+    if values and all(v == 0 and math.copysign(1, v) < 0 for v in values):
+        r.flags |= po.XF_ALL_NEGZERO
+    scale = 1 << po.EXACT_SCALE
+    for v in values:
+        if v != v:
+            r.flags |= po.XF_NAN
+        elif abs(v) == float("inf"):
+            r.flags |= po.XF_PINF if v > 0 else po.XF_NINF
+        elif v == 0:
+            r.flags |= po.XF_NEGZERO if math.copysign(1, v) < 0 else po.XF_POSZERO
+        else:
+            u = int(Fraction(v) * scale)
+            low = ((abs(u) & -abs(u)).bit_length() - 1) - po.EXACT_SCALE
+            r.lowbit = low if r.lowbit is None else min(r.lowbit, low)
+            r.s += u
+            r.a += abs(u)
+    return r
+
+
+def check_float8_agg(fn, x, values, ctx=()):
+    """a one-stage float8 SUM or AVG `x` over the non-NULL inputs `values`, held to _check_exact's rule"""
+    _check_exact(fn, False, 0, x, exact_record(values), tuple(ctx))
+
+
 def assert_aggrows_match(got, want, agg, rel=1e-6, float_exact=False, exact=None):
     """Integer results and keys bit-exact; float8 sums/avgs within `rel` (the tolerance BASELINE.json states).
 
