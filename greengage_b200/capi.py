@@ -259,6 +259,9 @@ def dev_lib():
         L.gg_groups_set_nonreceiver.restype = None
         L.gg_groups_free.argtypes = [vp]
         L.gg_groups_free.restype = None
+        L.gg_scanagg_datumrows.argtypes = [vp, C.POINTER(vp), C.POINTER(u64)]
+        L.gg_joinagg_datumrows.argtypes = [vp, C.POINTER(vp), C.POINTER(u64)]
+        L.gg_groups_datumrows.argtypes = [vp, C.POINTER(vp), C.POINTER(u64)]
         L.gg_ic_unique_id.argtypes = [vp, i32]
         L.gg_ic_create.argtypes = [vp, vp, i32, i32, C.POINTER(vp)]
         L.gg_ic_teardown.argtypes = [vp, i32]

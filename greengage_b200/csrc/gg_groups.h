@@ -38,6 +38,10 @@ struct gg_groups {
 	uint8_t keytype[GG_MAX_KEYS];
 	uint8_t acckind[GGP_MAX_ACCS];
 	int32_t keytypid[GG_MAX_KEYS];            /* type OIDs of the grouping columns */
+	/* gg_groups_datumrows: the finalised groups as datum rows (owned by this object, also when it is a view) */
+	gg_relation *rows_buf = nullptr;
+	gg_relation *rows_view = nullptr;
+	uint64_t rows_n = 0;
 };
 
 /* a new owned set with the metadata of `like` */

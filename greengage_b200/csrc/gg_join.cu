@@ -377,6 +377,17 @@ int gg_joinagg_fetch(gg_joinagg *j, gg_aggrow *out, int outcap, int *nout, uint6
 	return gg_scanagg_fetch(j->probe, out, outcap, nout, nullptr, rows_joined);
 }
 
+/* the joined-and-aggregated groups as datum rows: the last pass as gg_joinagg_fetch runs it, then the probe pipeline's rows */
+int gg_joinagg_datumrows(gg_joinagg *j, gg_relation **rows, uint64_t *nrows)
+{
+	if (!j) return GG_ERR_ARG;
+	if (j->ntargets) { gg_set_error("a join with a target list returns rows (gg_joinagg_rows), not aggregate rows"); return GG_ERR_ARG; }
+	if (j->bj && j->nbatch > 1) return gg_scanagg_datumrows(j->bj->probe, rows, nrows);     /* every batch was filled as it went */
+	int rc = joinagg_fill_inner(j);
+	if (rc) return rc;
+	return gg_scanagg_datumrows(j->probe, rows, nrows);
+}
+
 /* ---- hybrid hash join: batches (nodeHash.c:713 ExecHashIncreaseNumBatches, :1132 ExecHashGetBucketAndBatch) ----
  * When the hash table of the whole inner side would not fit the operator's memory, both inputs are split by the batch bits
  * of the join's hash value — the reference's hash function (per key: rotate left one bit, xor the key type's hash function,

@@ -70,6 +70,10 @@ struct gg_scanagg {
 	/* set by a batched join: how to feed the inputs again (its batches, each with its own hash table) when fetch has to
 	 * replay them on a wider kernel variant; empty: replay `fed` */
 	std::function<int()> replay_hook;
+	/* gg_scanagg_datumrows: the finalised groups as datum rows (owned, grown as needed) and the view handed out (until reset) */
+	gg_relation *rows_buf = nullptr;
+	gg_relation *rows_view = nullptr;
+	uint64_t rows_n = 0;
 	/* host staging for the streamed path */
 	uint8_t *stage[2] = { nullptr, nullptr };
 	cudaEvent_t ev_copied[2] = { nullptr, nullptr }, ev_consumed[2] = { nullptr, nullptr };
@@ -82,6 +86,11 @@ int scanagg_launch(gg_scanagg *p, const uint8_t *dev_pages, uint64_t nblocks, cu
 /* reset the pipeline and feed its inputs again (through replay_hook when set) on kernel variant `mode` (MODE_HASH: a group
  * table of ha_cap slots) */
 extern "C" int scanagg_replay(gg_scanagg *p, int mode, uint64_t ha_cap);
+/* Bring the pipeline to its final state, as gg_scanagg_fetch and gg_scanagg_datumrows find it: wait for everything queued,
+ * apply the join's build error, and escalate (PRIV -> TR / TRN -> HASH -> HASH x 8) and replay until the variant holds every
+ * group.  *flags, *nmerged (the merged records of a block-table variant) and counters[2] (rows scanned / passed) are the
+ * status it ends with; the flags are not yet turned into an error. */
+extern "C" int scanagg_settle(gg_scanagg *p, uint32_t *flags, int *nmerged, unsigned long long counters[2]);
 /* gg_motion.cu: the partitioning kernel behind gg_motion_partition, with the routing rule as a parameter (route 0: segments by
  * cdbhash + jump consistent hash; route 1: hash-join batches by the batch bits above `shift`) */
 int gg_partition_rows(gg_engine *e, const gg_scan *scan, const gg_exprpool *pool,

@@ -286,6 +286,7 @@ gg_merge_recs_kernel(const ggp_grec *recs, int nrecs, int nkeys, uint32_t keytyp
 
 #include "gg_pipeline.h"
 #include "gg_groups.h"
+#include "gg_aggfinal.h"
 
 static_assert(sizeof(BlockTable) == GG_BLOCKTABLE_BYTES && GG_REG_GROUPS == 4, "gg_launch.h sizes the shared memory with these");
 static_assert((int) GGL_PRIV == MODE_PRIV && (int) GGL_TR == MODE_TR && (int) GGL_TRN == MODE_TRN && (int) GGL_BUILD == MODE_BUILD &&
@@ -564,6 +565,7 @@ int gg_scanagg_reset(gg_scanagg *p)
 	GG_CUDA(cudaMemsetAsync(p->merged, 0, sizeof(ggp_grec) * GG_MERGE_CAP, st));
 	GG_CUDA(cudaMemsetAsync(p->d_status, 0, sizeof(gg_scanagg::Status), st));
 	if (p->mo.cursor) GG_CUDA(cudaMemsetAsync(p->mo.cursor, 0, sizeof(unsigned long long), st));
+	if (p->rows_view) { gg_relation_free(p->rows_view); p->rows_view = nullptr; }
 	p->has_state = false;
 	p->kev_used = 0;
 	if (p->mode == MODE_HASH)
@@ -812,19 +814,20 @@ static int finalize_rows(const gg_agg *agg, const ggp_aggmap *aggmap, const uint
 				continue;
 			}
 			uint64_t nn = x.n[col];
-			int64_t ibits;
-			memcpy(&ibits, &x.sum[col], 8);
+			uint64_t acc;
+			memcpy(&acc, &x.sum[col], 8);
+			if (gg_aggfinal_covers(fn) && !(partial && fn == GG_AGG_AVG_FLOAT8))
+			{
+				/* the rule the device applies when it writes the group as a datum row (gg_aggfinal.h) */
+				int isnull = 0;
+				const uint64_t w = gg_aggfinal(fn, x.count, nn, acc, &isnull);
+				v.isnull = isnull;
+				if (gg_aggfinal_is_float8(fn)) memcpy(&v.f[0], &w, 8);
+				else v.i = (int64_t) w;
+				continue;
+			}
 			switch (fn)
 			{
-				case GG_AGG_COUNT_ANY:
-					v.i = (int64_t) nn;
-					break;
-				case GG_AGG_SUM_FLOAT8:
-				case GG_AGG_MIN_FLOAT8:
-				case GG_AGG_MAX_FLOAT8:
-					v.isnull = nn == 0;
-					v.f[0] = nn ? x.sum[col] : 0.0;
-					break;
 				case GG_AGG_SUM_NUMERIC:
 				case GG_AGG_AVG_NUMERIC:
 				{
@@ -847,20 +850,9 @@ static int finalize_rows(const gg_agg *agg, const ggp_aggmap *aggmap, const uint
 					}
 					break;
 				}
-				case GG_AGG_AVG_FLOAT8:
-					if (partial)
-					{
-						/* float8_accum's state starts from "{0,0,0}": + 0.0 turns the -0 the sums start from into +0 */
-						v.f[0] = (double) nn; v.f[1] = x.sum[col] + 0.0; v.f[2] = x.sumsq[col] + 0.0;
-					}
-					else if (nn == 0)
-						v.isnull = 1;            /* float8_avg: N == 0 => NULL (float.c:1995) */
-					else
-						v.f[0] = (x.sum[col] + 0.0) / (double) nn;
-					break;
-				default:                      /* int sum/min/max */
-					v.isnull = nn == 0;
-					v.i = nn ? ibits : 0;
+				case GG_AGG_AVG_FLOAT8:      /* PARTIAL: the transition state */
+					/* float8_accum's state starts from "{0,0,0}": + 0.0 turns the -0 the sums start from into +0 */
+					v.f[0] = (double) nn; v.f[1] = x.sum[col] + 0.0; v.f[2] = x.sumsq[col] + 0.0;
 					break;
 			}
 		}
@@ -909,39 +901,53 @@ int scanagg_replay(gg_scanagg *p, int mode, uint64_t ha_cap)
 	return GG_OK;
 }
 
+int scanagg_settle(gg_scanagg *p, uint32_t *flags, int *nmerged, unsigned long long counters[2])
+{
+	gg_engine *e = p->eng;
+	GG_CUDA(cudaSetDevice(e->device));
+	for (;;)
+	{
+		GG_CUDA(cudaStreamSynchronize(e->copy_stream));
+		/* one round trip: status words and (speculatively) the first merged group records, behind everything queued */
+		GG_CUDA(cudaMemcpyAsync(&p->h_mirror->st, p->d_status, sizeof(gg_scanagg::Status), cudaMemcpyDeviceToHost, e->stream));
+		GG_CUDA(cudaMemcpyAsync(p->h_mirror->recs, p->recs, sizeof p->h_mirror->recs, cudaMemcpyDeviceToHost, e->stream));
+		GG_CUDA(cudaStreamSynchronize(e->stream));
+		*flags = p->h_mirror->st.err;
+		counters[0] = p->h_mirror->st.counters[0];
+		counters[1] = p->h_mirror->st.counters[1];
+		*nmerged = p->h_mirror->st.nout;
+		if (p->build_err)
+		{
+			const int brc = gg_errflags_to_code(p->build_err);        /* the join's hash table holds a value the device refused */
+			if (brc) return brc;
+		}
+		/* Escalation, then the inputs are replayed and looked at again.  Private accumulators: more groups than they hold (the
+		 * planner's numGroups was low or absent), or a non-finite private sum, which only the value-tracking transposed variant
+		 * can attribute to an infinite input or to a float8pl overflow.  A block-table variant with more groups than a block
+		 * holds: the general HashAggregate.  Its table full: one 8 times larger. */
+		int next = -1;
+		uint64_t cap = 0;
+		if (p->mode == MODE_PRIV && (*flags & (GGP_EF_GROUP_OVERFLOW | GGP_EF_RECHECK))) next = p->prog.nullable ? MODE_TRN : MODE_TR;
+		else if (p->mode != MODE_HASH && (*flags & GGP_EF_GROUP_OVERFLOW)) { next = MODE_HASH; cap = p->ha_cap ? p->ha_cap : 1u << 20; }
+		else if (p->mode == MODE_HASH && (*flags & GGP_EF_TABLE_FULL)) { next = MODE_HASH; cap = p->ha_cap * 8; }
+		if (next < 0) return GG_OK;
+		if (cap > (1ull << 31)) { gg_set_error("more groups than the device hash aggregate can hold"); return GG_ERR_NOMEM; }
+		int rc = scanagg_replay(p, next, cap);
+		if (rc) return rc;
+	}
+}
+
 int gg_scanagg_fetch(gg_scanagg *p, gg_aggrow *out, int outcap, int *nout,
                      uint64_t *rows_scanned, uint64_t *rows_passed)
 {
 	if (!p || !nout) return GG_ERR_ARG;
 	gg_engine *e = p->eng;
-	GG_CUDA(cudaSetDevice(e->device));
-	GG_CUDA(cudaStreamSynchronize(e->copy_stream));
-	/* one round trip: status words and (speculatively) the first merged group records, behind everything queued */
-	GG_CUDA(cudaMemcpyAsync(&p->h_mirror->st, p->d_status, sizeof(gg_scanagg::Status), cudaMemcpyDeviceToHost, e->stream));
-	GG_CUDA(cudaMemcpyAsync(p->h_mirror->recs, p->recs, sizeof p->h_mirror->recs, cudaMemcpyDeviceToHost, e->stream));
-	GG_CUDA(cudaStreamSynchronize(e->stream));
-	uint32_t flags = p->h_mirror->st.err;
-	unsigned long long counters[2] = { p->h_mirror->st.counters[0], p->h_mirror->st.counters[1] };
-	int n = p->h_mirror->st.nout;
-	if (p->build_err)
+	uint32_t flags = 0;
+	unsigned long long counters[2] = { 0, 0 };
+	int n = 0;
 	{
-		const int brc = gg_errflags_to_code(p->build_err);        /* the join's hash table holds a value the device refused */
-		if (brc) return brc;
-	}
-	/* Escalation, then the inputs are replayed and fetched again.  Private accumulators: more groups than they hold (the
-	 * planner's numGroups was low or absent), or a non-finite private sum, which only the value-tracking transposed variant can
-	 * attribute to an infinite input or to a float8pl overflow.  A block-table variant with more groups than a block holds:
-	 * the general HashAggregate.  Its table full: one 8 times larger. */
-	int next = -1;
-	uint64_t cap = 0;
-	if (p->mode == MODE_PRIV && (flags & (GGP_EF_GROUP_OVERFLOW | GGP_EF_RECHECK))) next = p->prog.nullable ? MODE_TRN : MODE_TR;
-	else if (p->mode != MODE_HASH && (flags & GGP_EF_GROUP_OVERFLOW)) { next = MODE_HASH; cap = p->ha_cap ? p->ha_cap : 1u << 20; }
-	else if (p->mode == MODE_HASH && (flags & GGP_EF_TABLE_FULL)) { next = MODE_HASH; cap = p->ha_cap * 8; }
-	if (next >= 0)
-	{
-		if (cap > (1ull << 31)) { gg_set_error("more groups than the device hash aggregate can hold"); return GG_ERR_NOMEM; }
-		int rc = scanagg_replay(p, next, cap);
-		return rc ? rc : gg_scanagg_fetch(p, out, outcap, nout, rows_scanned, rows_passed);
+		const int src = scanagg_settle(p, &flags, &n, counters);
+		if (src) return src;
 	}
 	if (rows_scanned) *rows_scanned = counters[0];
 	if (rows_passed) *rows_passed = counters[1];
@@ -1017,6 +1023,8 @@ void gg_scanagg_free(gg_scanagg *p)
 	cudaStreamSynchronize(p->eng->stream);
 	cudaFree(p->recs); cudaFree(p->merged); cudaFree(p->vidx); cudaFree(p->vmap);
 	cudaFree(p->d_status); cudaFreeHost(p->h_mirror); cudaFree(p->d_nout64); cudaFree(p->ha_mem); cudaFree(p->d_aocs);
+	if (p->rows_view) gg_relation_free(p->rows_view);
+	if (p->rows_buf) gg_relation_free(p->rows_buf);
 	for (int b = 0; b < 2; b++)
 	{
 		if (p->stage[b]) cudaFree(p->stage[b]);
@@ -1130,6 +1138,7 @@ gg_groups *gg_groups_alloc(gg_engine *e, const gg_groups *like, int cap, bool sp
 	gg_groups *g = new gg_groups();
 	if (like) *g = *like;
 	g->eng = e; g->cap = cap; g->sparse = sparse; g->owned = true;
+	g->rows_buf = nullptr; g->rows_view = nullptr; g->rows_n = 0;      /* `like`'s rows are its own */
 	const int alloc_cap = cap <= GG_GROUPS_POOL_CAP ? GG_GROUPS_POOL_CAP : cap;
 	void *mem = nullptr;
 	if (alloc_cap == GG_GROUPS_POOL_CAP && !e->groups_pool.empty()) { mem = e->groups_pool.back(); e->groups_pool.pop_back(); }
@@ -1147,6 +1156,8 @@ extern "C" {
 void gg_groups_free(gg_groups *g)
 {
 	if (!g) return;
+	if (g->rows_view) gg_relation_free(g->rows_view);
+	if (g->rows_buf) gg_relation_free(g->rows_buf);
 	if (g->owned && g->recs)
 	{
 		/* stream-ordered reuse: whoever takes the buffer next works on the same stream */

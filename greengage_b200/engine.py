@@ -131,6 +131,21 @@ def motion_partition(eng, scan, pool, hashkeys, payload, nsegs, rel, out_ptr, ou
     return list(counts), list(offs)
 
 
+def _datumrows(fn, h, ncols):
+    """the datum rows an Agg's gg_*_datumrows hands out, read to the host: (values int64 [n][ncols], isnull bool [n][ncols])"""
+    rel, n = C.c_void_p(), C.c_uint64(0)
+    check(fn(h, C.byref(rel), C.byref(n)))
+    n = n.value
+    W = 1 + ncols
+    nb = (n * W * 8 + capi.GG_BLCKSZ - 1) // capi.GG_BLCKSZ
+    buf = np.zeros(nb * capi.GG_BLCKSZ // 8, dtype=np.uint64)
+    if nb:
+        check(dev_lib().gg_relation_read(rel, 0, buf.ctypes.data, nb))
+    r = buf[:n * W].reshape(n, W)
+    nulls = ((r[:, :1] >> np.arange(ncols, dtype=np.uint64)) & np.uint64(1)).astype(bool)
+    return np.ascontiguousarray(r[:, 1:]).view(np.int64), nulls
+
+
 class ScanAgg:
     """SeqScan -> qual -> Agg pipeline (gg_scanagg)."""
 
@@ -173,6 +188,10 @@ class ScanAgg:
         buf = np.frombuffer(self._raw, dtype=np.uint8, count=n.value * C.sizeof(capi.gg_aggrow))
         return buf, n.value, sc.value, ps.value
 
+    def datumrows(self):
+        """the groups finalised on the device (gg_scanagg_datumrows), in the order the device wrote them: (values, isnull)"""
+        return _datumrows(dev_lib().gg_scanagg_datumrows, self.h, self.agg.numCols + self.agg.numAggs)
+
     def scan_kernel_ms(self):
         ms, n = C.c_float(0), C.c_int(0)
         check(dev_lib().gg_scanagg_scan_kernel_ms(self.h, C.byref(ms), C.byref(n)))
@@ -193,6 +212,7 @@ class JoinAgg:
     def __init__(self, eng, outer, inner, hj, agg, pool):
         self.eng = eng
         self.h = C.c_void_p()
+        self.agg = agg
         check(dev_lib().gg_joinagg_create(eng.h, C.byref(outer), C.byref(inner), C.byref(hj), C.byref(agg), C.byref(pool),
                                           C.byref(self.h)))
 
@@ -225,6 +245,10 @@ class JoinAgg:
         nj = C.c_uint64(0)
         check(dev_lib().gg_joinagg_fetch(self.h, out, cap, C.byref(n), C.byref(nj)))
         return [out[i] for i in range(n.value)], nj.value
+
+    def datumrows(self):
+        """the joined-and-aggregated groups finalised on the device (gg_joinagg_datumrows): (values, isnull)"""
+        return _datumrows(dev_lib().gg_joinagg_datumrows, self.h, self.agg.numCols + self.agg.numAggs)
 
     def stats(self):
         rb, tb = C.c_uint64(0), C.c_uint64(0)
@@ -322,6 +346,10 @@ class Groups:
         h = C.c_void_p()
         check(dev_lib().gg_groups_final(self.eng.h, self.h, C.byref(h)))
         return Groups(self.eng, h)
+
+    def datumrows(self, ncols):
+        """the groups finalised on the device (gg_groups_datumrows): (values, isnull) of ncols = numCols + numAggs columns"""
+        return _datumrows(dev_lib().gg_groups_datumrows, self.h, ncols)
 
     def fetch(self, cap=4096):
         out = (capi.gg_aggrow * cap)()

@@ -40,6 +40,10 @@ enum { K_SCANAGG = 1, K_JOINAGG, K_AGGFINAL, K_SORT, K_MOTION, K_SCANROWS, K_HAS
 /* the same for the join that writes its rows: without them a HashJoin with a target list is refused (GG_ERR_UNSUPPORTED) */
 #pragma weak gg_joinrows_create
 #pragma weak gg_joinagg_rows
+/* the same for the Agg that finalises its groups into datum rows: without them an Agg under a Sort or a Limit hands up host rows */
+#pragma weak gg_scanagg_datumrows
+#pragma weak gg_joinagg_datumrows
+#pragma weak gg_groups_datumrows
 
 struct GgPlanState {
 	int kind;
@@ -78,6 +82,9 @@ struct GgPlanState {
 	int nonreceiver;                    /* above a Gather, on a segment that is not its receiver: no rows at all */
 	int dev_groups;                     /* decided at init, from the plan alone (so every segment decides alike): this node hands
 	                                     * its aggregate rows up as device-resident group records */
+	int agg_rows;                       /* decided at init, from the plan alone: an Agg directly under a Sort or a Limit hands up its
+	                                     * groups finalised into device datum rows (rows_rel), which the node above sorts or windows
+	                                     * where they are */
 	int lazy_fetch;                     /* set by a Motion above that moves this node's records on the device: the pipeline's result
 	                                     * is not fetched to the host before it travels (no host synchronisation between the scan
 	                                     * and the Motion); what a fetch would have decided travels as status flags */
@@ -132,8 +139,8 @@ const char *GgExecNodeKind(GgPlanState *s)
 const char *GgExecNodeResultLocation(GgPlanState *s)
 {
 	if (!s || !s->done) return "";
-	if (s->groups && !s->rows_ready) return "device-groups";
 	if (s->rows_rel && !s->rows_ready) return "device-rows";
+	if (s->groups && !s->rows_ready) return "device-groups";
 	return "host";
 }
 
@@ -482,6 +489,21 @@ static int init_join(GgPlanState *s, GgPlan *node, const gg_agg *agg, int eflags
 	return 0;
 }
 
+/* An Agg directly under a Sort or a Limit finalises its groups on the device into datum rows, which the node above sorts or
+ * windows in place (only the Limit's window comes to the host).  Decided from the plan alone, so every segment decides alike:
+ * a one-stage Agg over a scan or a join, or a FINAL Agg that combines device group records; no numeric aggregate (finalised on
+ * the host only); and a device library with the entry points.  Otherwise the Agg hands up host rows, as it always did. */
+static void mark_agg_rows(GgPlanState *ch)
+{
+	int i, ok;
+	if (!gg_scanagg_datumrows || !gg_joinagg_datumrows || !gg_groups_datumrows) return;
+	ok = ((ch->kind == K_SCANAGG || ch->kind == K_JOINAGG) && ch->agg.aggstage == GG_AGGSTAGE_NORMAL) ||
+	     (ch->kind == K_AGGFINAL && ch->dev_groups);
+	for (i = 0; ok && i < ch->agg.numAggs; i++)
+		ok = ch->agg.aggs[i].aggfnoid != GG_AGG_SUM_NUMERIC && ch->agg.aggs[i].aggfnoid != GG_AGG_AVG_NUMERIC;
+	ch->agg_rows = ok && ch->agg.numCols + ch->agg.numAggs > 0;
+}
+
 static GgPlanState *init_node(GgPlan *node, GgEState *estate, int eflags, int depth)
 {
 	GgPlanState *s;
@@ -551,6 +573,7 @@ static GgPlanState *init_node(GgPlan *node, GgEState *estate, int eflags, int de
 			s->sort_bound = GG_NO_BOUND;
 			s->child = init_node(node->lefttree, estate, eflags, depth + 1);
 			if (!s->child) goto fail;
+			mark_agg_rows(s->child);
 			return s;
 		}
 		case T_GgLimit:
@@ -560,6 +583,7 @@ static GgPlanState *init_node(GgPlan *node, GgEState *estate, int eflags, int de
 			s->kind = K_LIMIT;
 			s->child = init_node(node->lefttree, estate, eflags, depth + 1);
 			if (!s->child) goto fail;
+			mark_agg_rows(s->child);
 			return s;
 		case T_GgMotion:
 		{
@@ -884,7 +908,7 @@ static int run_rows_node(GgPlanState *s)
 /* the device buffer that holds a rows node's datum rows */
 static gg_relation *rows_buffer(const GgPlanState *s)
 {
-	if (s->kind == K_JOINROWS) return s->rows_rel;        /* the join's own output buffer */
+	if (s->kind == K_JOINROWS || s->agg_rows) return s->rows_rel;        /* the join's / the Agg's own output buffer */
 	return s->rows_recv && s->rows_nsegs > 1 ? s->rows_recv : s->rows_send;
 }
 
@@ -924,6 +948,31 @@ static int rows_to_host(GgPlanState *s)
 	return 0;
 }
 
+/* a failure reading a node's aggregate rows: this segment's own earlier failure, when there was one, is the better message */
+static void groups_fail(const GgPlanState *s, int rc)
+{
+	if (s->groups && g_local_code && rc != GG_ERR_RETRY_HOST) exec_fail(g_local_code, "%s", g_local_err);
+	else exec_fail(rc, "%s", gg_last_error());
+}
+
+/* the Agg's groups as device datum rows (agg_rows): the view its pipeline or group set hands out, wrapped for the node above */
+static int agg_datumrows(GgPlanState *s)
+{
+	gg_relation *out = NULL;
+	int rc;
+	if (set_layout_types(s)) return -1;
+	if (s->groups) rc = gg_groups_datumrows(s->groups, &out, &s->rows_n);
+	else if (s->kind == K_SCANAGG) rc = gg_scanagg_datumrows(s->sa, &out, &s->rows_n);
+	else rc = gg_joinagg_datumrows(s->ja, &out, &s->rows_n);
+	if (rc != GG_OK) { groups_fail(s, rc); return -1; }
+	s->rows_ncols = s->ncols;
+	s->rows_nsegs = 1;
+	rc = gg_relation_attach_rows(s->estate->engine, gg_relation_device_ptr(out), s->rows_n, s->rows_ncols, &s->rows_rel);
+	if (rc != GG_OK) { s->rows_rel = NULL; exec_fail(rc, "%s", gg_last_error()); return -1; }
+	s->rows_ready = 0;
+	return 0;
+}
+
 /* a node's aggregate rows -> host result arrays, from its device group records (the one synchronisation of a
  * device-resident slice) or else from its scan / join pipeline */
 static int aggrows_to_host(GgPlanState *s)
@@ -942,8 +991,7 @@ static int aggrows_to_host(GgPlanState *s)
 	}
 	if (rc != GG_OK)
 	{
-		if (s->groups && g_local_code && rc != GG_ERR_RETRY_HOST) exec_fail(g_local_code, "%s", g_local_err);      /* this segment's own failure */
-		else exec_fail(rc, "%s", gg_last_error());
+		groups_fail(s, rc);
 		free(rows);
 		return -1;
 	}
@@ -963,8 +1011,8 @@ static int pipeline_groups(GgPlanState *s)
 static int ensure_rows(GgPlanState *s)
 {
 	if (s->rows_ready) return 0;
-	if (s->groups) return aggrows_to_host(s);
 	if (s->rows_rel || s->kind == K_SCANROWS || (s->kind == K_MOTION && s->rows_scan)) return rows_to_host(s);
+	if (s->groups) return aggrows_to_host(s);
 	exec_fail(GG_ERR_ARG, "node has no result");
 	return -1;
 }
@@ -1122,6 +1170,8 @@ static int run_agg_pipeline(GgPlanState *s)
 		return 0;
 	}
 	if (rc != GG_OK) { exec_fail(rc, "%s", gg_last_error()); return -1; }
+	/* under a Sort / Limit: the groups are settled (as a fetch settles them) and finalised into datum rows on the device */
+	if (s->agg_rows) return agg_datumrows(s);
 	if (s->lazy_fetch && !es->motion_on_host && pipeline_groups(s) == GG_OK)
 	{
 		/* the records go straight into the Motion above; a pipeline that would have to be replayed says so in its
@@ -1152,6 +1202,7 @@ static int run_final_agg(GgPlanState *s)
 	{
 		rc = gg_groups_final(es->engine, ch->groups, &s->groups);
 		if (rc != GG_OK) { exec_fail(rc, "%s", gg_last_error()); return -1; }
+		if (s->agg_rows) return agg_datumrows(s);
 		if (set_layout_types(s)) return -1;
 		s->rows_ready = 0;
 		return 0;

@@ -16,6 +16,8 @@
  *     Agg <- HashJoin(SeqScan, Hash(SeqScan)) build kernel + probe kernel   (gg_joinagg_*)
  *     HashJoin with a target list             build kernel + row-writing probe: datum rows (gg_joinrows_create)
  *     Sort <- any of the above                device radix sort             (gg_sort_rows)
+ *     Sort / Limit <- Agg                      the groups finalised into device datum rows and sorted / windowed there
+ *                                             (gg_scanagg_datumrows, gg_joinagg_datumrows, gg_groups_datumrows)
  *     Motion <- any of the above              rows handed to the transport  (GgMotionTransport)
  * and returns NULL with GgExecLastError() set when a node or a shape is outside the accelerated subset, so the
  * caller keeps the CPU nodes for that subtree (there is no CPU implementation behind this API).

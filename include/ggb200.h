@@ -247,6 +247,21 @@ int  gg_groups_final(gg_engine *e, gg_groups *in, gg_groups **out);
  * stage says (PARTIAL: transition states; otherwise finalised values). */
 int  gg_groups_fetch(gg_groups *g, gg_aggrow *out, int outcap, int *nout, uint64_t *rows_scanned, uint64_t *rows_passed);
 int  gg_groups_info(gg_groups *g, int *sparse, int *cap);
+/* ---- aggregate rows as datum rows ----
+ * The groups of an Agg finalised on the device (finalize_aggregate, nodeAgg.c:871-999) into GG_FMT_DATUMROWS rows that a Sort
+ * or a Limit above takes where they are (gg_sort_datumrows*): word 0 the NULL mask (bit c: grouping column c, bit numCols + i:
+ * aggregate i), then the numCols grouping keys, then one word per aggregate — bit for bit what the *_fetch calls put into a
+ * gg_aggrow's key[c] and agg[i].f[0] (float8 results) or agg[i].i.  No slot is dead.  Order: that of *_fetch for the merged
+ * records of a block-table variant and for a group set; for the general HashAggregate a function of its table's contents
+ * (unspecified, as for a hash aggregate).  A plain aggregate over no input still gives its one row (not on a segment that does
+ * not receive a Gather).  The pipeline is settled first exactly as *_fetch settles it (kernel-variant escalation and replay,
+ * the join's build error, the fill-inner pass of right / full joins), with fetch's error codes and messages.
+ * *rows is a view owned by the pipeline or the set, valid until its reset or free; the buffer is 16-byte aligned with 16 bytes
+ * of slack and grows as needed.  GG_ERR_UNSUPPORTED: a PARTIAL stage (its consumers read group records) or a numeric
+ * aggregate (finalised on the host only). */
+int  gg_scanagg_datumrows(gg_scanagg *p, gg_relation **rows, uint64_t *nrows);
+int  gg_joinagg_datumrows(gg_joinagg *j, gg_relation **rows, uint64_t *nrows);
+int  gg_groups_datumrows(gg_groups *g, gg_relation **rows, uint64_t *nrows);
 void gg_groups_set_nonreceiver(gg_groups *g);
 void gg_groups_free(gg_groups *g);
 
