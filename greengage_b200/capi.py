@@ -262,6 +262,10 @@ def dev_lib():
         L.gg_scanagg_datumrows.argtypes = [vp, C.POINTER(vp), C.POINTER(u64)]
         L.gg_joinagg_datumrows.argtypes = [vp, C.POINTER(vp), C.POINTER(u64)]
         L.gg_groups_datumrows.argtypes = [vp, C.POINTER(vp), C.POINTER(u64)]
+        L.gg_rowfilter_create.argtypes = [vp, C.POINTER(gg_tupdesc), C.c_int32, C.POINTER(gg_exprpool), C.POINTER(vp)]
+        L.gg_rowfilter_run.argtypes = [vp, vp, u64, C.POINTER(vp), C.POINTER(u64)]
+        L.gg_rowfilter_free.argtypes = [vp]
+        L.gg_rowfilter_free.restype = None
         L.gg_ic_unique_id.argtypes = [vp, i32]
         L.gg_ic_create.argtypes = [vp, vp, i32, i32, C.POINTER(vp)]
         L.gg_ic_teardown.argtypes = [vp, i32]

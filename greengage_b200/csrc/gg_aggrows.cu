@@ -13,6 +13,9 @@
  *   the HBM hash table         of the general HashAggregate, read in place: an order-preserving compaction over the table's
  *                              slots — per-tile counts, the exclusive scan of gg_sort.cu, per-tile writes — so the row order
  *                              is a function of the table's contents, with no atomics deciding it
+ *
+ * And the row filter of an Agg's HAVING (gg_rowfilter_*): the same order-preserving compaction over datum rows, with the
+ * interpreter deciding which rows pass.
  */
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -164,10 +167,101 @@ gg_aggrows_write_kernel(const Src src, uint64_t nslots, const uint32_t *cnt, con
 	}
 }
 
+/* ---- the row filter (gg_rowfilter_*): an Agg's HAVING over its datum rows, order-preserving ----
+ * pass 1  a tile of RF_TILE rows, RF_THREADS at a time, is copied coalesced into shared memory (odd word stride: the lanes read
+ *         their own rows from distinct banks); every thread runs the interpreter over its row (datumrow_passes); one pass bit per
+ *         row, one count per tile
+ * pass 2  the exclusive scan of the counts (gg_scan_*)
+ * pass 3  every tile copies its passing rows, in row order, from its exclusive prefix on: placement is a function of the input */
+#define RF_THREADS 256
+#define RF_ITEMS   8
+#define RF_TILE    (RF_THREADS * RF_ITEMS)
+
+__global__ void __launch_bounds__(RF_THREADS)
+gg_rowfilter_count_kernel(const __grid_constant__ ggp_program P, const unsigned long long *rows, uint64_t n, uint32_t W, uint32_t *bits,
+                          uint32_t *cnt, uint32_t *errflags)
+{
+	extern __shared__ __align__(16) unsigned long long s_rows[];
+	__shared__ uint32_t s_warp[RF_THREADS / 32];
+	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+	const uint32_t S = W | 1u;
+	uint32_t c = 0, err = 0;
+	for (int k = 0; k < RF_ITEMS; k++)
+	{
+		const uint64_t base = (uint64_t) blockIdx.x * RF_TILE + (uint64_t) k * RF_THREADS;
+		if (base >= n) break;                                              /* the same for the whole block */
+		const uint32_t m = n - base < RF_THREADS ? (uint32_t) (n - base) : RF_THREADS;
+		const unsigned long long *src = rows + base * W;
+		__syncthreads();
+		for (uint32_t j = threadIdx.x; j < m * W; j += RF_THREADS)
+		{
+			const uint32_t r = j / W;
+			s_rows[r * S + (j - r * W)] = src[j];
+		}
+		__syncthreads();
+		const bool present = threadIdx.x < m;
+		const bool pass = datumrow_passes(P, smem_u32(s_rows + (present ? threadIdx.x : 0) * S), present, lane, err);
+		const unsigned b = __ballot_sync(GG_FULL_MASK, pass);
+		if (lane == 0) bits[(base >> 5) + warp] = b;
+		c += pass ? 1u : 0u;
+	}
+	if (err) atomicOr(errflags, err);
+	for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(GG_FULL_MASK, c, o);
+	if (lane == 0) s_warp[warp] = c;
+	__syncthreads();
+	if (threadIdx.x == 0)
+	{
+		uint32_t t = 0;
+		for (int w = 0; w < RF_THREADS / 32; w++) t += s_warp[w];
+		cnt[blockIdx.x] = t;
+	}
+}
+
+__global__ void __launch_bounds__(RF_THREADS)
+gg_rowfilter_write_kernel(const unsigned long long *rows, uint64_t n, uint32_t W, const uint32_t *bits, const uint32_t *cnt,
+                          unsigned long long *out)
+{
+	__shared__ uint32_t s_warp[RF_THREADS / 32];
+	__shared__ uint16_t s_idx[RF_THREADS];
+	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+	uint64_t at = cnt[blockIdx.x];
+	for (int k = 0; k < RF_ITEMS; k++)
+	{
+		const uint64_t base = (uint64_t) blockIdx.x * RF_TILE + (uint64_t) k * RF_THREADS;
+		if (base >= n) break;
+		const unsigned b = bits[(base >> 5) + warp];
+		if (lane == 0) s_warp[warp] = __popc(b);
+		__syncthreads();
+		uint32_t pre = 0, tot = 0;
+		for (int w = 0; w < RF_THREADS / 32; w++) { const uint32_t s = s_warp[w]; pre += w < warp ? s : 0; tot += s; }
+		if ((b >> lane) & 1u) s_idx[pre + __popc(b & ((1u << lane) - 1u))] = (uint16_t) threadIdx.x;
+		__syncthreads();
+		/* the survivors' words, written contiguously */
+		unsigned long long *dst = out + at * W;
+		for (uint32_t j = threadIdx.x; j < tot * W; j += RF_THREADS)
+		{
+			const uint32_t r = j / W;
+			dst[j] = rows[(base + s_idx[r]) * W + (j - r * W)];
+		}
+		at += tot;
+		__syncthreads();                                                   /* s_warp / s_idx are reused */
+	}
+}
+
 /* the exclusive scan of gg_sort.cu over m counters (three phases over chunks of 4096) */
 __global__ void gg_scan_sums_kernel(const uint32_t *x, uint64_t m, uint32_t *sums);
 __global__ void gg_scan_top_kernel(uint32_t *sums, uint32_t nblk);
 __global__ void gg_scan_apply_kernel(uint32_t *x, uint64_t m, const uint32_t *sums);
+
+struct gg_rowfilter {
+	gg_engine *eng = nullptr;
+	ggp_program prog;                    /* ggp_compile_filter */
+	int ncols = 0;                       /* columns of the rows filtered (a row is 1 + ncols words) */
+	uint32_t *scratch = nullptr;         /* error word, tile counts, scan sums, pass bits; grown as needed */
+	uint64_t scratch_words = 0;
+	gg_relation *rows_buf = nullptr;     /* the survivors (owned) */
+	gg_relation *rows_view = nullptr;    /* the view handed out */
+};
 
 /* =====================================================================================
  * host side
@@ -357,6 +451,98 @@ int gg_groups_datumrows(gg_groups *g, gg_relation **rows, uint64_t *nrows)
 	*rows = g->rows_view;
 	*nrows = g->rows_n;
 	return GG_OK;
+}
+
+int gg_rowfilter_create(gg_engine *e, const gg_tupdesc *rows_desc, int32_t qual, const gg_exprpool *pool, gg_rowfilter **out)
+{
+	if (!e || !rows_desc || !pool || !out) return GG_ERR_ARG;
+	*out = nullptr;
+	gg_scan scan;
+	memset(&scan, 0, sizeof scan);
+	scan.desc = *rows_desc;
+	scan.qual = qual;
+	gg_rowfilter *f = new gg_rowfilter();
+	char msg[256];
+	const int rc = ggp_compile_filter(&scan, pool, &f->prog, msg, sizeof msg);
+	if (rc != GG_OK) { gg_set_error("HAVING: %s", msg); delete f; return rc; }
+	f->eng = e;
+	f->ncols = rows_desc->natts;
+	*out = f;
+	return GG_OK;
+}
+
+int gg_rowfilter_run(gg_rowfilter *f, gg_relation *rows, uint64_t nrows, gg_relation **out_view, uint64_t *nout)
+{
+	if (!f || !rows || !out_view || !nout) return GG_ERR_ARG;
+	const uint64_t W = 1 + (uint64_t) f->ncols;
+	if ((uint64_t) rows->rowwords != W) { gg_set_error("row filter over %d columns: the relation has rows of %d words", f->ncols, rows->rowwords); return GG_ERR_ARG; }
+	if (nrows > rows->nrows) { gg_set_error("row filter: %llu rows of a relation of %llu", (unsigned long long) nrows, (unsigned long long) rows->nrows); return GG_ERR_ARG; }
+	gg_engine *e = f->eng;
+	cudaStream_t st = e->stream;
+	GG_CUDA(cudaSetDevice(e->device));
+	uint32_t total = 0;
+	if (nrows)
+	{
+		/* scratch: the error word, ntiles + 1 counters (the last one becomes the total), the scan's block sums, the pass bits */
+		const uint64_t ntiles = (nrows + RF_TILE - 1) / RF_TILE;
+		const uint64_t m = ntiles + 1;
+		const uint32_t nblk = (uint32_t) ((m + 4095) / 4096);
+		const uint64_t words = 1 + m + nblk + ntiles * (RF_TILE / 32);
+		if (f->scratch_words < words)
+		{
+			cudaFree(f->scratch);
+			f->scratch = nullptr;
+			f->scratch_words = 0;
+			const cudaError_t ce = cudaMalloc((void **) &f->scratch, (size_t) words * 4);
+			if (ce != cudaSuccess) { cudaGetLastError(); gg_set_error("row filter: scratch of %llu words does not fit in device memory", (unsigned long long) words); return GG_ERR_NOMEM; }
+			f->scratch_words = words;
+		}
+		uint32_t *d_err = f->scratch, *cnt = f->scratch + 1, *sums = cnt + m, *bits = sums + nblk;
+		const unsigned long long *in = (const unsigned long long *) rows->pages;
+		const int smem = RF_THREADS * (int) (W | 1) * 8;
+		GG_CUDA(cudaFuncSetAttribute(gg_rowfilter_count_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+		GG_CUDA(cudaMemsetAsync(f->scratch, 0, (size_t) (1 + m) * 4, st));
+		gg_rowfilter_count_kernel<<<(unsigned) ntiles, RF_THREADS, smem, st>>>(f->prog, in, nrows, (uint32_t) W, bits, cnt, d_err);
+		gg_scan_sums_kernel<<<nblk, 256, 0, st>>>(cnt, m, sums);
+		gg_scan_top_kernel<<<1, 256, 0, st>>>(sums, nblk);
+		gg_scan_apply_kernel<<<nblk, 256, 0, st>>>(cnt, m, sums);
+		e->launches += 4;
+		GG_CUDA(cudaGetLastError());
+		uint32_t flags = 0;
+		GG_CUDA(cudaMemcpyAsync(&flags, d_err, 4, cudaMemcpyDeviceToHost, st));
+		GG_CUDA(cudaMemcpyAsync(&total, cnt + ntiles, 4, cudaMemcpyDeviceToHost, st));
+		GG_CUDA(cudaStreamSynchronize(st));
+		const int rc = gg_errflags_to_code(flags);
+		if (rc != GG_OK) return rc;
+		int r2 = reserve_rows(e, &f->rows_buf, total, W);
+		if (r2) return r2;
+		if (total)
+		{
+			gg_rowfilter_write_kernel<<<(unsigned) ntiles, RF_THREADS, 0, st>>>(in, nrows, (uint32_t) W, bits, cnt, (unsigned long long *) f->rows_buf->pages);
+			e->launches++;
+			GG_CUDA(cudaGetLastError());
+		}
+	}
+	else
+	{
+		const int rc = reserve_rows(e, &f->rows_buf, 0, W);
+		if (rc) return rc;
+	}
+	const int rc = rows_view(e, f->rows_buf, total, f->ncols, &f->rows_view);
+	if (rc) return rc;
+	*out_view = f->rows_view;
+	*nout = total;
+	return GG_OK;
+}
+
+void gg_rowfilter_free(gg_rowfilter *f)
+{
+	if (!f) return;
+	if (f->eng) cudaSetDevice(f->eng->device);
+	if (f->rows_view) gg_relation_free(f->rows_view);
+	if (f->rows_buf) gg_relation_free(f->rows_buf);
+	cudaFree(f->scratch);
+	delete f;
 }
 
 }  /* extern "C" */

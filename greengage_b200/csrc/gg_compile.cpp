@@ -1177,6 +1177,29 @@ int ggp_compile_joinrows(const gg_scan *outer, const gg_scan *inner, const gg_ha
 	return compile_join(outer, inner, hj, nullptr, targets, ntargets, pool, jp, nullptr, err, errlen);
 }
 
+/* An Agg's HAVING (nodeAgg.c:1092 ExecQual over the finalised group, gg_rowfilter): the qual of a scan of the Agg's output rows,
+ * nothing else.  The rows are GG_FMT_DATUMROWS; Vars are varno 0, varattno = output column (keys, then aggregates). */
+int ggp_compile_filter(const gg_scan *scan, const gg_exprpool *pool, ggp_program *prog, char *err, int errlen)
+{
+	Ctx c;
+	memset(prog, 0, sizeof *prog);
+	memset(&c, 0, sizeof c);
+	c.pool = pool; c.prog = prog; c.outer = &prog->outer; c.odesc = &scan->desc; c.err = err; c.errlen = errlen;
+	if (err && errlen) err[0] = 0;
+	if (scan->desc.format != GG_FMT_DATUMROWS) { fail(c, "a row filter reads datum rows (GG_FMT_DATUMROWS)"); return GG_ERR_ARG; }
+	if (scan->desc.natts < 1) { fail(c, "a row filter over rows without columns"); return GG_ERR_ARG; }
+	{
+		Roots roots;
+		if (!valid_header(c, pool, &scan->desc, nullptr)) return GG_ERR_ARG;
+		roots.add(c, pool, scan->qual, false, "qual");
+		if (!roots.ok || !valid_nodes(c, pool, &scan->desc, nullptr, roots)) return GG_ERR_ARG;
+	}
+	init_side(&prog->outer, &scan->desc);
+	gen_qual(c, scan->qual);
+	if (!c.failed) emit(c, GGP_END);
+	return c.failed ? GG_ERR_UNSUPPORTED : GG_OK;
+}
+
 /* Redistribute Motion (nodeMotion.c:1481-1687): which tuples go where, and what travels */
 int ggp_compile_motion(const gg_scan *scan, const gg_exprpool *pool, const int32_t *hashkeys, int nkeys,
                        const int32_t *payload, int npayload, ggp_program *prog, uint8_t *hashtype,

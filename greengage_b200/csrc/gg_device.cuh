@@ -784,4 +784,36 @@ __device__ __forceinline__ void run_prog(const EvalCtx &X, bool live, uint32_t &
 	run_range<NULLABLE, HAS_INNER>(X, M, 0, GGP_MAX_CODE, err, sink);
 }
 
+/* the sink of a program that only filters (ggp_compile_filter): the row passes when every FILTER saw TRUE */
+struct FilterSink {
+	bool pass;
+	__device__ __forceinline__ bool filter(bool p) { pass = p; return p; }
+	__device__ __forceinline__ void key(int, uint64_t, bool) {}
+	__device__ __forceinline__ bool group(bool l) { return l; }
+	__device__ __forceinline__ void out(int, double, bool) {}
+};
+/* An Agg's HAVING over one datum row at shared address rp (NULL mask word, then one word per column; the front end of the scan
+ * kernels' datum rows): TRUE passes, FALSE and NULL do not (ExecQual), a dead slot never does.  Errors of the rows that are
+ * evaluated go to err; an arm the reference skips raises nothing (GGP_GUARD_*). */
+__device__ __forceinline__ bool datumrow_passes(const ggp_program &P, uint32_t rp, bool present, int lane, uint32_t &err)
+{
+	EvalCtx X;
+	const uint64_t mask = present ? lds64(rp) : GG_DATUMROW_DEAD;
+	const bool live = !(mask & GG_DATUMROW_DEAD);
+	uint32_t cn = 0;
+	for (int sl = 0; sl < P.outer.ncols; sl++) cn |= (uint32_t) ((mask >> P.outer.colatt[sl]) & 1) << sl;
+	X.P = &P;
+	X.tv.tp = rp + 8;
+	X.tv.colnull = live ? cn : 0;
+	X.offs = 0;
+	X.fast = true;
+	X.ipay = nullptr;
+	X.ipaynull = 0;
+	X.lane = lane;
+	FilterSink sink;
+	sink.pass = live;
+	run_prog<true, false>(X, live, err, sink);
+	return sink.pass;
+}
+
 }  // namespace ggd

@@ -249,6 +249,8 @@ int ggp_compile_join(const gg_scan *outer, const gg_scan *inner, const gg_hashjo
  * an output row) and one OUT per target (1..16, Vars with varno 0 outer / 1 inner) */
 int ggp_compile_joinrows(const gg_scan *outer, const gg_scan *inner, const gg_hashjoin *hj, const int32_t *targets, int ntargets,
                          const gg_exprpool *pool, ggp_joinprog *jp, char *err, int errlen);
+/* Row filter (an Agg's HAVING over its finalised rows): scan->qual as FILTERs over the GG_FMT_DATUMROWS scan->desc, then END */
+int ggp_compile_filter(const gg_scan *scan, const gg_exprpool *pool, ggp_program *prog, char *err, int errlen);
 #endif
 
 #endif /* GG_PROGRAM_H */

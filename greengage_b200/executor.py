@@ -157,9 +157,11 @@ class PlanBuilder:
             n.targets[i] = t
         return n
 
-    def agg(self, child, agg):
+    def agg(self, child, agg, having=-1):
+        """having: the HAVING qual's expression root (Vars varno 0, varattno = 1-based output column of the Agg: grouping keys,
+        then one per aggregate); -1 = none"""
         n = self._keep(GgAgg())
-        n.plan.type, n.plan.qual, n.plan.lefttree = T_Agg, -1, _as_plan(child)
+        n.plan.type, n.plan.qual, n.plan.lefttree = T_Agg, having, _as_plan(child)
         C.memmove(C.byref(n.agg), C.byref(agg), C.sizeof(capi.gg_agg))
         return n
 

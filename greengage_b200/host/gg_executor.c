@@ -44,6 +44,13 @@ enum { K_SCANAGG = 1, K_JOINAGG, K_AGGFINAL, K_SORT, K_MOTION, K_SCANROWS, K_HAS
 #pragma weak gg_scanagg_datumrows
 #pragma weak gg_joinagg_datumrows
 #pragma weak gg_groups_datumrows
+/* the row filter of an Agg's HAVING: without it (or without the three above) an Agg with a qual is refused (GG_ERR_UNSUPPORTED);
+ * no path runs the Agg with its qual dropped */
+#pragma weak gg_rowfilter_create
+#pragma weak gg_rowfilter_run
+#pragma weak gg_rowfilter_free
+/* and the upload of a FINAL Agg's host-finalised rows to such a filter or to a join */
+#pragma weak gg_relation_load
 
 struct GgPlanState {
 	int kind;
@@ -82,9 +89,12 @@ struct GgPlanState {
 	int nonreceiver;                    /* above a Gather, on a segment that is not its receiver: no rows at all */
 	int dev_groups;                     /* decided at init, from the plan alone (so every segment decides alike): this node hands
 	                                     * its aggregate rows up as device-resident group records */
-	int agg_rows;                       /* decided at init, from the plan alone: an Agg directly under a Sort or a Limit hands up its
-	                                     * groups finalised into device datum rows (rows_rel), which the node above sorts or windows
-	                                     * where they are */
+	int agg_rows;                       /* decided at init, from the plan alone: an Agg directly under a Sort or a Limit, under a
+	                                     * HashJoin, or with a HAVING qual hands up its groups finalised into device datum rows
+	                                     * (rows_rel), which the node above sorts, windows or joins where they are */
+	gg_rowfilter *having;               /* an Agg's plan.qual (HAVING), compiled at init over its rows_desc */
+	int rows_required;                  /* an Agg under a HashJoin: the join reads device rows only, so a FINAL Agg whose groups were
+	                                     * finalised on the host uploads them */
 	int lazy_fetch;                     /* set by a Motion above that moves this node's records on the device: the pipeline's result
 	                                     * is not fetched to the host before it travels (no host synchronisation between the scan
 	                                     * and the Motion); what a fetch would have decided travels as status flags */
@@ -326,6 +336,7 @@ static void end_tree(GgPlanState *s)
 	if (s->rows_recv) gg_relation_free(s->rows_recv);
 	if (s->sa) gg_scanagg_free(s->sa);
 	if (s->ja) gg_joinagg_free(s->ja);
+	if (s->having) gg_rowfilter_free(s->having);
 	free(s->values); free(s->isnull); free(s->lens);
 	free(s);
 }
@@ -369,9 +380,32 @@ static int bind_relation(GgEState *es, const GgSeqScan *scan, gg_relation **rel,
 /* what a scan or join pipeline reads: a SeqScan's relation, or the datum rows of a row-producing node */
 static int is_pipeline_input(const GgPlan *p) { return p && (p->type == T_GgSeqScan || yields_rows(p)); }
 
+/* a join also reads the groups of an Agg, finalised into device datum rows (init_input checks that it can deliver them) */
+static int is_join_input(const GgPlan *p) { return is_pipeline_input(p) || (p && p->type == T_GgAgg); }
+
+static void mark_agg_rows(GgPlanState *ch);
+static int agg_rows_desc(GgPlanState *s);
+
 static int init_input(GgPlanState *s, GgPlan *p, int eflags, int depth, gg_scan *scan, GgPlanState **rows, gg_relation **rel)
 {
 	memset(scan, 0, sizeof *scan);
+	if (p->type == T_GgAgg)
+	{
+		/* an Agg under a HashJoin hands up its groups as device rows, by the rule of an Agg under a Sort (mark_agg_rows) */
+		GgPlanState *ch;
+		if (!(ch = *rows = init_node(p, s->estate, eflags, depth))) return -1;
+		mark_agg_rows(ch);
+		if (!ch->agg_rows || !gg_relation_load)
+		{
+			exec_fail(GG_ERR_UNSUPPORTED, "HashJoin over an Agg: only a one-stage Agg over a scan or a join, or a FINAL Agg over device "
+			          "group records, without numeric aggregates, delivers its groups as device rows");
+			return -1;
+		}
+		if (!ch->having && agg_rows_desc(ch)) return -1;
+		ch->rows_required = 1;
+		scan->desc = ch->rows_desc; scan->qual = -1;
+		return 0;
+	}
 	if (yields_rows(p))
 	{
 		if (!(*rows = init_node(p, s->estate, eflags, depth))) return -1;
@@ -447,9 +481,10 @@ static int init_join(GgPlanState *s, GgPlan *node, const gg_agg *agg, int eflags
 	{ exec_fail(GG_ERR_UNSUPPORTED, "HashJoin with a target list: the device library has no join that writes its rows"); return -1; }
 	if (!agg && (hj->numTargets > GG_MAX_OUTCOLS || hj->numTargets > 16))
 	{ exec_fail(GG_ERR_UNSUPPORTED, "HashJoin projecting %d columns (1..16 travel as datum rows)", hj->numTargets); return -1; }
-	if (!hash || hash->type != T_GgHash || !is_pipeline_input(outer) || !is_pipeline_input(inner))
+	if (!hash || hash->type != T_GgHash || !is_join_input(outer) || !is_join_input(inner))
 	{
-		exec_fail(GG_ERR_UNSUPPORTED, "HashJoin: both inputs must be a SeqScan or a Redistribute Motion over one (Hash on the inner side)");
+		exec_fail(GG_ERR_UNSUPPORTED, "HashJoin: both inputs must be a SeqScan, a Redistribute Motion over one, a HashJoin with a target "
+		          "list or an Agg (Hash on the inner side)");
 		return -1;
 	}
 	s->kind = agg ? K_JOINAGG : K_JOINROWS;
@@ -489,19 +524,71 @@ static int init_join(GgPlanState *s, GgPlan *node, const gg_agg *agg, int eflags
 	return 0;
 }
 
+static int has_numeric_agg(const gg_agg *agg)
+{
+	int i;
+	for (i = 0; i < agg->numAggs; i++)
+		if (agg->aggs[i].aggfnoid == GG_AGG_SUM_NUMERIC || agg->aggs[i].aggfnoid == GG_AGG_AVG_NUMERIC) return 1;
+	return 0;
+}
+
 /* An Agg directly under a Sort or a Limit finalises its groups on the device into datum rows, which the node above sorts or
  * windows in place (only the Limit's window comes to the host).  Decided from the plan alone, so every segment decides alike:
  * a one-stage Agg over a scan or a join, or a FINAL Agg that combines device group records; no numeric aggregate (finalised on
  * the host only); and a device library with the entry points.  Otherwise the Agg hands up host rows, as it always did. */
 static void mark_agg_rows(GgPlanState *ch)
 {
-	int i, ok;
+	int ok;
+	if (ch->having) return;                      /* decided at its own init: it always hands up (filtered) device rows */
 	if (!gg_scanagg_datumrows || !gg_joinagg_datumrows || !gg_groups_datumrows) return;
 	ok = ((ch->kind == K_SCANAGG || ch->kind == K_JOINAGG) && ch->agg.aggstage == GG_AGGSTAGE_NORMAL) ||
 	     (ch->kind == K_AGGFINAL && ch->dev_groups);
-	for (i = 0; ok && i < ch->agg.numAggs; i++)
-		ok = ch->agg.aggs[i].aggfnoid != GG_AGG_SUM_NUMERIC && ch->agg.aggs[i].aggfnoid != GG_AGG_AVG_NUMERIC;
-	ch->agg_rows = ok && ch->agg.numCols + ch->agg.numAggs > 0;
+	ch->agg_rows = ok && !has_numeric_agg(&ch->agg) && ch->agg.numCols + ch->agg.numAggs > 0;
+}
+
+/* The GG_FMT_DATUMROWS descriptor of an Agg's finalised rows: its output columns as set_layout_types types them.  NOT NULL
+ * only where it is certain: count(*) and count(x) are never NULL; a key or any other aggregate may be (a NULL grouping value,
+ * an aggregate over no non-NULL input).  A wrong NOT NULL would select a consumer's NULL-free kernel variant over NULLs. */
+static int agg_rows_desc(GgPlanState *s)
+{
+	int c;
+	if (set_layout_types(s)) return -1;
+	if (s->ncols > GG_MAX_ATTS) { exec_fail(GG_ERR_UNSUPPORTED, "Agg with %d output columns (datum rows carry up to %d)", s->ncols, GG_MAX_ATTS); return -1; }
+	memset(&s->rows_desc, 0, sizeof s->rows_desc);
+	s->rows_desc.natts = s->ncols;
+	s->rows_desc.format = GG_FMT_DATUMROWS;
+	for (c = 0; c < s->ncols; c++)
+	{
+		gg_attr *a = &s->rows_desc.attrs[c];
+		const int i = c - s->agg.numCols;
+		a->atttypid = s->typid[c]; a->atttypmod = -1; a->attlen = 8; a->attalign = 'd'; a->attbyval = 1;
+		a->attnotnull = i >= 0 && (s->agg.aggs[i].aggfnoid == GG_AGG_COUNT_STAR || s->agg.aggs[i].aggfnoid == GG_AGG_COUNT_ANY);
+	}
+	s->rows_ncols = s->ncols;
+	return 0;
+}
+
+/* An Agg's HAVING (plan.qual; nodeAgg.c:1092 ExecQual over every finalised group).  Decided from the plan alone, so every
+ * segment decides alike: the Agg always hands up its groups as device datum rows, filtered by the qual on the device
+ * (gg_rowfilter); a FINAL Agg whose groups end up finalised on the host uploads them once and filters them the same way.  What
+ * cannot take that path is refused: no path runs the Agg with its qual dropped. */
+static int init_having(GgPlanState *s, int32_t qual)
+{
+	int rc;
+	if (s->agg.aggstage == GG_AGGSTAGE_PARTIAL)
+	{ exec_fail(GG_ERR_UNSUPPORTED, "a PARTIAL-stage Agg with a qual (HAVING belongs to the stage that finalises the groups)"); return -1; }
+	if (has_numeric_agg(&s->agg))
+	{ exec_fail(GG_ERR_UNSUPPORTED, "Agg with a qual: numeric aggregates have no device datum row to filter"); return -1; }
+	if (s->agg.numCols + s->agg.numAggs < 1) { exec_fail(GG_ERR_UNSUPPORTED, "Agg with a qual and no output columns"); return -1; }
+	if (!gg_rowfilter_create || !gg_rowfilter_run || !gg_rowfilter_free || !gg_relation_load || !gg_scanagg_datumrows || !gg_joinagg_datumrows ||
+	    !gg_groups_datumrows)
+	{ exec_fail(GG_ERR_UNSUPPORTED, "Agg with a qual: the device library has no row filter or no aggregate datum rows"); return -1; }
+	if (agg_rows_desc(s)) return -1;
+	rc = gg_rowfilter_create(s->estate->engine, &s->rows_desc, qual, s->estate->pool, &s->having);
+	if (rc != GG_OK) { s->having = NULL; exec_fail(rc, "Agg qual: %s", gg_last_error()); return -1; }
+	s->agg_rows = 1;
+	if (s->kind != K_AGGFINAL) s->dev_groups = 0;     /* a FINAL Agg keeps dev_groups: it says how it combines its input */
+	return 0;
 }
 
 static GgPlanState *init_node(GgPlan *node, GgEState *estate, int eflags, int depth)
@@ -544,13 +631,13 @@ static GgPlanState *init_node(GgPlan *node, GgEState *estate, int eflags, int de
 					for (i = 0; same && i < an->agg.numAggs; i++) same = ch->agg.aggs[i].aggfnoid == an->agg.aggs[i].aggfnoid;
 					s->dev_groups = same;
 				}
-				return s;
+				goto agg_qual;
 			}
 			/* a HashJoin directly below stays fused with this Agg, whether it has a target list or not */
 			if (below && below->type == T_GgHashJoin)
 			{
 				if (init_join(s, below, &an->agg, eflags, depth)) goto fail;
-				return s;
+				goto agg_qual;
 			}
 			if (is_pipeline_input(below))
 			{
@@ -560,10 +647,13 @@ static GgPlanState *init_node(GgPlan *node, GgEState *estate, int eflags, int de
 				rc = gg_scanagg_create(estate->engine, &scan, &an->agg, estate->pool, &s->sa);
 				if (rc != GG_OK) { exec_fail(rc, "Agg <- SeqScan: %s", gg_last_error()); goto fail; }
 				s->dev_groups = 1;
-				return s;
+				goto agg_qual;
 			}
 			exec_fail(GG_ERR_UNSUPPORTED, "Agg: child node type %d is not on the accelerated path", below ? (int) below->type : 0);
 			goto fail;
+		agg_qual:
+			if (node->qual != -1 && init_having(s, node->qual)) goto fail;
+			return s;
 		}
 		case T_GgSort:
 		{
@@ -599,7 +689,7 @@ static GgPlanState *init_node(GgPlan *node, GgEState *estate, int eflags, int de
 			{
 				/* aggregate rows move as device-resident group records when the rows below are such records, the hash columns
 				 * are grouping columns, and the receiver does not merge sorted streams */
-				int c, ok = estate->interconnect != NULL && s->child->dev_groups && mo->numSortCols == 0;
+				int c, ok = estate->interconnect != NULL && s->child->dev_groups && !s->child->having && mo->numSortCols == 0;
 				for (c = 0; ok && mo->motionType == GG_MOTIONTYPE_HASH && c < mo->numHashCols; c++)
 					ok = mo->hashCol[c] >= 0 && mo->hashCol[c] < s->child->agg.numCols;
 				s->dev_groups = ok;
@@ -955,6 +1045,20 @@ static void groups_fail(const GgPlanState *s, int rc)
 	else exec_fail(rc, "%s", gg_last_error());
 }
 
+/* an Agg's s->rows_n finalised rows (a datum-row view) handed up as s->rows_rel: through its HAVING filter first, when it has one,
+ * so that only the groups whose qual is TRUE reach the node above */
+static int hand_up_rows(GgPlanState *s, gg_relation *rows)
+{
+	int rc = GG_OK;
+	s->rows_ncols = s->ncols;
+	s->rows_nsegs = 1;
+	if (s->having) rc = gg_rowfilter_run(s->having, rows, s->rows_n, &rows, &s->rows_n);
+	if (rc == GG_OK) rc = gg_relation_attach_rows(s->estate->engine, gg_relation_device_ptr(rows), s->rows_n, s->rows_ncols, &s->rows_rel);
+	if (rc != GG_OK) { s->rows_rel = NULL; exec_fail(rc, "%s", gg_last_error()); return -1; }
+	s->rows_ready = 0;
+	return 0;
+}
+
 /* the Agg's groups as device datum rows (agg_rows): the view its pipeline or group set hands out, wrapped for the node above */
 static int agg_datumrows(GgPlanState *s)
 {
@@ -965,12 +1069,39 @@ static int agg_datumrows(GgPlanState *s)
 	else if (s->kind == K_SCANAGG) rc = gg_scanagg_datumrows(s->sa, &out, &s->rows_n);
 	else rc = gg_joinagg_datumrows(s->ja, &out, &s->rows_n);
 	if (rc != GG_OK) { groups_fail(s, rc); return -1; }
-	s->rows_ncols = s->ncols;
-	s->rows_nsegs = 1;
-	rc = gg_relation_attach_rows(s->estate->engine, gg_relation_device_ptr(out), s->rows_n, s->rows_ncols, &s->rows_rel);
-	if (rc != GG_OK) { s->rows_rel = NULL; exec_fail(rc, "%s", gg_last_error()); return -1; }
-	s->rows_ready = 0;
-	return 0;
+	return hand_up_rows(s, out);
+}
+
+/* A FINAL Agg whose groups were finalised on the host (its child delivered host rows, or the slice was re-run with host-row
+ * Motions), under a HAVING filter or a HashJoin: its host rows uploaded once as datum rows (into rows_send) and handed up as the
+ * device path hands them up, so the qual is evaluated one way only */
+static int upload_agg_rows(GgPlanState *s)
+{
+	GgEState *es = s->estate;
+	const uint64_t n = s->nrows > 0 ? (uint64_t) s->nrows : 0, W = 1 + (uint64_t) s->ncols;
+	const uint64_t nb = (n * W * 8 + 16 + GG_BLCKSZ - 1) / GG_BLCKSZ;
+	gg_relation *view = NULL;
+	uint64_t *buf, r;
+	int c, rc;
+	if (s->rows_send && gg_relation_nblocks(s->rows_send) < nb) { gg_relation_free(s->rows_send); s->rows_send = NULL; }
+	if (!s->rows_send && (rc = gg_relation_create(es->engine, nb, &s->rows_send)) != GG_OK)
+	{ s->rows_send = NULL; exec_fail(rc, "Agg rows: %s", gg_last_error()); return -1; }
+	buf = calloc((size_t) nb, GG_BLCKSZ);
+	if (!buf) { exec_fail(GG_ERR_NOMEM, "out of memory"); return -1; }
+	for (r = 0; r < n; r++)
+		for (c = 0; c < s->ncols; c++)
+		{
+			buf[r * W] |= (uint64_t) (s->isnull[r * (uint64_t) s->ncols + c] != 0) << c;
+			buf[r * W + 1 + c] = (uint64_t) s->values[r * (uint64_t) s->ncols + c];
+		}
+	rc = gg_relation_load(s->rows_send, 0, buf, nb);              /* pageable: staged before the call returns, so buf can go */
+	free(buf);
+	if (rc == GG_OK) rc = gg_relation_attach_rows(es->engine, gg_relation_device_ptr(s->rows_send), n, s->ncols, &view);
+	if (rc != GG_OK) { exec_fail(rc, "Agg rows: %s", gg_last_error()); return -1; }
+	s->rows_n = n;
+	rc = hand_up_rows(s, view);
+	gg_relation_free(view);
+	return rc;
 }
 
 /* a node's aggregate rows -> host result arrays, from its device group records (the one synchronisation of a
@@ -1214,6 +1345,7 @@ static int run_final_agg(GgPlanState *s)
 		 * even the empty-input row of a plain aggregate */
 		if (alloc_result(s, 0, ch->ncols)) { exec_fail(GG_ERR_NOMEM, "out of memory"); return -1; }
 		s->rows_ready = 1;
+		if (s->having || s->rows_required) { if (set_layout_types(s)) return -1; s->nrows = 0; return upload_agg_rows(s); }
 		return 0;
 	}
 	part.aggstage = GG_AGGSTAGE_PARTIAL;      /* layout of the incoming rows */
@@ -1229,6 +1361,7 @@ static int run_final_agg(GgPlanState *s)
 	if (rc != GG_OK) { exec_fail(rc, "%s", gg_last_error()); free(out); return -1; }
 	rc = rows_from_aggrows(s, out, n);
 	free(out);
+	if (rc == 0 && (s->having || s->rows_required)) rc = upload_agg_rows(s);
 	return rc;
 }
 

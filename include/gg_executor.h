@@ -18,6 +18,9 @@
  *     Sort <- any of the above                device radix sort             (gg_sort_rows)
  *     Sort / Limit <- Agg                      the groups finalised into device datum rows and sorted / windowed there
  *                                             (gg_scanagg_datumrows, gg_joinagg_datumrows, gg_groups_datumrows)
+ *     Agg with HAVING (plan.qual)             its groups as device datum rows, filtered on the device (gg_rowfilter_run);
+ *                                             refused (GG_ERR_UNSUPPORTED) where that cannot run, never run without its qual
+ *     HashJoin <- Agg (either side)           the Agg's groups as device datum rows, scanned by the join like join rows
  *     Motion <- any of the above              rows handed to the transport  (GgMotionTransport)
  * and returns NULL with GgExecLastError() set when a node or a shape is outside the accelerated subset, so the
  * caller keeps the CPU nodes for that subtree (there is no CPU implementation behind this API).

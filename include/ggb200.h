@@ -262,6 +262,21 @@ int  gg_groups_info(gg_groups *g, int *sparse, int *cap);
 int  gg_scanagg_datumrows(gg_scanagg *p, gg_relation **rows, uint64_t *nrows);
 int  gg_joinagg_datumrows(gg_joinagg *j, gg_relation **rows, uint64_t *nrows);
 int  gg_groups_datumrows(gg_groups *g, gg_relation **rows, uint64_t *nrows);
+/* ---- row filter: an Agg's HAVING over its datum rows ----
+ * ExecQual of the Agg's plan.qual over every finalised group (nodeAgg.c:1092): a row passes only if the qual is TRUE (NULL
+ * does not pass); AND / OR skip the arm the reference skips, so it raises nothing.  rows_desc is the GG_FMT_DATUMROWS descriptor
+ * of the rows (for an Agg: its grouping keys, then one column per aggregate, typed as the Agg outputs them); qual is an
+ * expression root in the pool whose Vars are varno 0, varattno = 1-based column of the rows.  create compiles the qual:
+ * GG_ERR_UNSUPPORTED with a message for a function or a type the device does not evaluate (numeric columns have no datum
+ * row), GG_ERR_ARG for a root outside the pool or a Var outside the columns.
+ * run filters the first nrows rows of a datum-row relation of that many columns: *out_view receives the rows whose qual is
+ * TRUE, in input order and in the same format, dead slots (GG_DATUMROW_DEAD) dropped; *nout their number.  The view is owned
+ * by the filter, valid until its next run or free.  nrows == 0 launches nothing.  Errors of the qual (float8 overflow,
+ * division by zero, date out of range, ...) are the reference's codes. */
+typedef struct gg_rowfilter gg_rowfilter;
+int  gg_rowfilter_create(gg_engine *e, const gg_tupdesc *rows_desc, int32_t qual, const gg_exprpool *pool, gg_rowfilter **out);
+int  gg_rowfilter_run(gg_rowfilter *f, gg_relation *rows, uint64_t nrows, gg_relation **out_view, uint64_t *nout);
+void gg_rowfilter_free(gg_rowfilter *f);
 void gg_groups_set_nonreceiver(gg_groups *g);
 void gg_groups_free(gg_groups *g);
 
