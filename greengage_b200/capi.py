@@ -41,6 +41,20 @@ AGG_COUNT_ANY, AGG_COUNT_STAR = 2147, 2803
 AGG_AVG_NUMERIC, AGG_SUM_NUMERIC = 2103, 2114
 
 AGGSTAGE_NORMAL, AGGSTAGE_PARTIAL, AGGSTAGE_FINAL = 0, 1, 3
+
+# window functions (pg_proc.h:4874-4902) and frame options (parsenodes.h:495-517)
+WF_ROW_NUMBER, WF_RANK, WF_DENSE_RANK, WF_PERCENT_RANK, WF_CUME_DIST, WF_NTILE = 3100, 3101, 3102, 3103, 3104, 3105
+WF_LAG, WF_LAG_OFFSET, WF_LAG_DEFAULT, WF_LEAD, WF_LEAD_OFFSET, WF_LEAD_DEFAULT = 3106, 3107, 3108, 3109, 3110, 3111
+WF_FIRST_VALUE, WF_LAST_VALUE, WF_NTH_VALUE = 3112, 3113, 3114
+GG_MAX_WINFUNCS = 8
+FRAMEOPTION_NONDEFAULT, FRAMEOPTION_RANGE, FRAMEOPTION_ROWS, FRAMEOPTION_BETWEEN = 0x1, 0x2, 0x4, 0x8
+FRAMEOPTION_START_UNBOUNDED_PRECEDING, FRAMEOPTION_END_UNBOUNDED_PRECEDING = 0x10, 0x20
+FRAMEOPTION_START_UNBOUNDED_FOLLOWING, FRAMEOPTION_END_UNBOUNDED_FOLLOWING = 0x40, 0x80
+FRAMEOPTION_START_CURRENT_ROW, FRAMEOPTION_END_CURRENT_ROW = 0x100, 0x200
+FRAMEOPTION_START_VALUE_PRECEDING, FRAMEOPTION_END_VALUE_PRECEDING = 0x400, 0x800
+FRAMEOPTION_START_VALUE_FOLLOWING, FRAMEOPTION_END_VALUE_FOLLOWING = 0x1000, 0x2000
+FRAMEOPTION_DEFAULTS = FRAMEOPTION_RANGE | FRAMEOPTION_START_UNBOUNDED_PRECEDING | FRAMEOPTION_END_CURRENT_ROW
+ERR_WINDOW_ARG = -14
 JOIN_INNER, JOIN_LEFT, JOIN_FULL, JOIN_RIGHT, JOIN_SEMI, JOIN_ANTI, JOIN_LASJ_NOTIN = 0, 1, 2, 3, 4, 5, 6
 E_VAR, E_CONST, E_FUNC, E_AND, E_OR, E_NOT, E_ISNULL, E_ISNOTNULL = 1, 2, 3, 4, 5, 6, 7, 8
 
@@ -99,6 +113,31 @@ class gg_hashjoin(C.Structure):
 
 class gg_sortkey(C.Structure):
     _fields_ = [("col", C.c_int32), ("typid", C.c_int32), ("desc", C.c_int32), ("nulls_first", C.c_int32)]
+
+
+class gg_winfunc(C.Structure):
+    _fields_ = [("winfnoid", C.c_int32), ("wintype", C.c_int32), ("arg", C.c_int32 * 3), ("pad", C.c_int32)]
+
+
+class gg_window(C.Structure):
+    _fields_ = [("partNumCols", C.c_int32), ("partColIdx", C.c_int32 * GG_MAX_KEYS), ("ordNumCols", C.c_int32),
+                ("ordColIdx", C.c_int32 * GG_MAX_KEYS), ("frameOptions", C.c_int32), ("numFuncs", C.c_int32),
+                ("funcs", gg_winfunc * GG_MAX_WINFUNCS)]
+
+
+def make_window(part, order, frame, funcs):
+    """part / order: 0-based input columns; frame: FRAMEOPTION_* bits; funcs: (winfnoid, wintype, [arg roots]) each"""
+    w = gg_window()
+    w.partNumCols, w.ordNumCols, w.frameOptions, w.numFuncs = len(part), len(order), frame, len(funcs)
+    for i, c in enumerate(part):
+        w.partColIdx[i] = c
+    for i, c in enumerate(order):
+        w.ordColIdx[i] = c
+    for i, (fn, ty, args) in enumerate(funcs):
+        w.funcs[i].winfnoid, w.funcs[i].wintype = fn, ty
+        for a in range(3):
+            w.funcs[i].arg[a] = args[a] if a < len(args) else -1
+    return w
 
 
 class gg_snapshot(C.Structure):
@@ -266,6 +305,10 @@ def dev_lib():
         L.gg_rowfilter_run.argtypes = [vp, vp, u64, C.POINTER(vp), C.POINTER(u64)]
         L.gg_rowfilter_free.argtypes = [vp]
         L.gg_rowfilter_free.restype = None
+        L.gg_window_create.argtypes = [vp, C.POINTER(gg_tupdesc), C.POINTER(gg_window), C.POINTER(gg_exprpool), C.POINTER(vp)]
+        L.gg_window_run.argtypes = [vp, vp, u64, C.POINTER(vp), C.POINTER(u64)]
+        L.gg_window_free.argtypes = [vp]
+        L.gg_window_free.restype = None
         L.gg_ic_unique_id.argtypes = [vp, i32]
         L.gg_ic_create.argtypes = [vp, vp, i32, i32, C.POINTER(vp)]
         L.gg_ic_teardown.argtypes = [vp, i32]

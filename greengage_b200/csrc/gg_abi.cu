@@ -69,6 +69,7 @@ const char *gg_strerror(int code)
 		case GG_ERR_DATE_RANGE: return "date out of range for timestamp";
 		case GG_ERR_PEER: return "another segment reported an error";
 		case GG_ERR_RETRY_HOST: return "run the slice again with host-row Motions";
+		case GG_ERR_WINDOW_ARG: return "invalid argument for a window function";
 	}
 	return "unknown error";
 }

@@ -146,6 +146,37 @@ def _datumrows(fn, h, ncols):
     return np.ascontiguousarray(r[:, 1:]).view(np.int64), nulls
 
 
+class Window:
+    """WindowAgg over datum rows (gg_window): one output row per live input row, the input's columns then one per function."""
+
+    def __init__(self, eng, rows_desc, win, pool):
+        self.eng = eng
+        self.h = C.c_void_p()
+        self.ncols = rows_desc.natts + win.numFuncs
+        check(dev_lib().gg_window_create(eng.h, C.byref(rows_desc), C.byref(win), C.byref(pool), C.byref(self.h)))
+
+    def run_raw(self, rows, nrows=None):
+        """rows: a RowRelation; returns (view handle, number of rows), the view valid until the next run"""
+        view, n = C.c_void_p(), C.c_uint64(0)
+        check(dev_lib().gg_window_run(self.h, rows.h, rows.nrows if nrows is None else nrows, C.byref(view), C.byref(n)))
+        return view, n.value
+
+    def run(self, rows, nrows=None):
+        """the output rows read to the host: their words as uint64 [n][1 + ncols] (NULL mask, then the columns)"""
+        view, n = self.run_raw(rows, nrows)
+        W = 1 + self.ncols
+        nb = (n * W * 8 + capi.GG_BLCKSZ - 1) // capi.GG_BLCKSZ
+        buf = np.zeros(nb * capi.GG_BLCKSZ // 8, dtype=np.uint64)
+        if nb:
+            check(dev_lib().gg_relation_read(view, 0, buf.ctypes.data, nb))
+        return buf[:n * W].reshape(n, W).copy()
+
+    def free(self):
+        if self.h:
+            dev_lib().gg_window_free(self.h)
+            self.h = C.c_void_p()
+
+
 class RowFilter:
     """An Agg's HAVING over datum rows (gg_rowfilter): the rows whose qual is TRUE, in input order."""
 

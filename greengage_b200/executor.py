@@ -12,7 +12,7 @@ import numpy as np
 from . import capi
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-T_SeqScan, T_Agg, T_Hash, T_HashJoin, T_Sort, T_Motion, T_Limit = 1, 2, 3, 4, 5, 6, 7
+T_SeqScan, T_Agg, T_Hash, T_HashJoin, T_Sort, T_Motion, T_Limit, T_WindowAgg = 1, 2, 3, 4, 5, 6, 7, 8
 MOTION_GATHER, MOTION_HASH, MOTION_BROADCAST = 0, 1, 2
 GG_MAX_SORTKEYS = 4
 GG_MAX_OUTCOLS = capi.GG_MAX_KEYS + 3 * capi.GG_MAX_AGGS
@@ -56,6 +56,10 @@ class GgMotion(C.Structure):
 class GgLimit(C.Structure):
     _fields_ = [("plan", GgPlan), ("hasOffset", C.c_int32), ("hasCount", C.c_int32), ("limitOffset", C.c_int64),
                 ("limitCount", C.c_int64)]
+
+
+class GgWindowAgg(C.Structure):
+    _fields_ = [("plan", GgPlan), ("win", capi.gg_window)]
 
 
 class GgTupleTableSlot(C.Structure):
@@ -194,6 +198,16 @@ class PlanBuilder:
         n.plan.type, n.plan.qual, n.plan.lefttree = T_Limit, -1, _as_plan(child)
         n.hasCount, n.limitCount = (0, 0) if count is None else (1, count)
         n.hasOffset, n.limitOffset = (0, 0) if offset is None else (1, offset)
+        return n
+
+    def windowagg(self, child, part, ord, frame, funcs, qual=-1):
+        """WindowAgg over `child` (a Sort on the partition columns, then the order columns): part / ord are 0-based columns of
+        the child's rows, frame the FRAMEOPTION_* bits, funcs (winfnoid, wintype, [arg roots]) each; qual: a SubqueryScan's qual
+        over the output row (the child's columns, then one per function; Vars varno 0, 1-based), -1 = none"""
+        n = self._keep(GgWindowAgg())
+        n.plan.type, n.plan.qual, n.plan.lefttree = T_WindowAgg, qual, _as_plan(child)
+        w = capi.make_window(part, ord, frame, funcs)
+        C.memmove(C.byref(n.win), C.byref(w), C.sizeof(capi.gg_window))
         return n
 
     def motion(self, child, motion_type, hash_cols=(), motion_id=1, merge_keys=()):

@@ -28,7 +28,7 @@
 int32_t gg_cdbhash_route(const int32_t *typids, const int64_t *vals, const int32_t *lens, const int32_t *isnull,
                          int nkeys, int nsegs);      /* gg_motion_host.c */
 
-enum { K_SCANAGG = 1, K_JOINAGG, K_AGGFINAL, K_SORT, K_MOTION, K_SCANROWS, K_HASH, K_LIMIT, K_JOINROWS };
+enum { K_SCANAGG = 1, K_JOINAGG, K_AGGFINAL, K_SORT, K_MOTION, K_SCANROWS, K_HASH, K_LIMIT, K_JOINROWS, K_WINDOW };
 
 #define GG_NO_BOUND UINT64_MAX
 
@@ -51,6 +51,11 @@ enum { K_SCANAGG = 1, K_JOINAGG, K_AGGFINAL, K_SORT, K_MOTION, K_SCANROWS, K_HAS
 #pragma weak gg_rowfilter_free
 /* and the upload of a FINAL Agg's host-finalised rows to such a filter or to a join */
 #pragma weak gg_relation_load
+/* the window functions: without them a WindowAgg is refused (GG_ERR_UNSUPPORTED); no other path runs it */
+#pragma weak gg_window_create
+#pragma weak gg_window_run
+#pragma weak gg_window_free
+#pragma weak gg_engine_last_kernel_ms
 
 struct GgPlanState {
 	int kind;
@@ -92,7 +97,9 @@ struct GgPlanState {
 	int agg_rows;                       /* decided at init, from the plan alone: an Agg directly under a Sort or a Limit, under a
 	                                     * HashJoin, or with a HAVING qual hands up its groups finalised into device datum rows
 	                                     * (rows_rel), which the node above sorts, windows or joins where they are */
-	gg_rowfilter *having;               /* an Agg's plan.qual (HAVING), compiled at init over its rows_desc */
+	gg_rowfilter *having;               /* an Agg's plan.qual (HAVING), compiled at init over its rows_desc; a WindowAgg's qual */
+	gg_window_obj *win;                 /* K_WINDOW: the window functions, created at init over the child's rows */
+	float win_ms;                       /* K_WINDOW: CUDA-event time of the last gg_window_run */
 	int rows_required;                  /* an Agg under a HashJoin: the join reads device rows only, so a FINAL Agg whose groups were
 	                                     * finalised on the host uploads them */
 	int lazy_fetch;                     /* set by a Motion above that moves this node's records on the device: the pipeline's result
@@ -141,6 +148,7 @@ const char *GgExecNodeKind(GgPlanState *s)
 		case K_HASH: return "hash";
 		case K_LIMIT: return "limit";
 		case K_JOINROWS: return "joinrows";
+		case K_WINDOW: return "windowagg";
 	}
 	return "";
 }
@@ -337,6 +345,7 @@ static void end_tree(GgPlanState *s)
 	if (s->sa) gg_scanagg_free(s->sa);
 	if (s->ja) gg_joinagg_free(s->ja);
 	if (s->having) gg_rowfilter_free(s->having);
+	if (s->win) gg_window_free(s->win);
 	free(s->values); free(s->isnull); free(s->lens);
 	free(s);
 }
@@ -354,11 +363,12 @@ GgPlanState *GgExecInitNode(GgPlan *node, GgEState *estate, int eflags)
 
 static int multi_segment(const GgEState *es) { return es->nsegs > 1; }
 
-/* a node that delivers device-resident datum rows: a SeqScan with a target list, a Motion over one, or a HashJoin with a
- * target list */
+/* a node that delivers device-resident datum rows: a SeqScan with a target list, a Motion over one, a HashJoin with a
+ * target list, or a WindowAgg */
 static int yields_rows(const GgPlan *p)
 {
 	if (!p) return 0;
+	if (p->type == T_GgWindowAgg) return 1;
 	if (p->type == T_GgSeqScan) return ((const GgSeqScan *) p)->numTargets > 0;
 	if (p->type == T_GgHashJoin) return ((const GgHashJoin *) p)->numTargets > 0;
 	if (p->type == T_GgMotion) return p->lefttree && p->lefttree->type == T_GgSeqScan && ((const GgSeqScan *) p->lefttree)->numTargets > 0;
@@ -591,6 +601,105 @@ static int init_having(GgPlanState *s, int32_t qual)
 	return 0;
 }
 
+/* The GG_FMT_DATUMROWS descriptor of the rows a node hands up, known at init: a row producer's own, an Agg's output columns,
+ * and through a Sort, a Limit or a Motion that of the node below */
+static int node_rows_desc(GgPlanState *s, gg_tupdesc *d)
+{
+	if (s->kind == K_SORT || s->kind == K_LIMIT || (s->kind == K_MOTION && !s->rows_scan)) return node_rows_desc(s->child, d);
+	if ((s->kind == K_SCANAGG || s->kind == K_JOINAGG || s->kind == K_AGGFINAL) && !s->having)
+	{
+		/* the descriptor of its output columns (a HAVING's init made it already); an Agg that hands up host rows keeps no row width */
+		if (agg_rows_desc(s)) return -1;
+		if (!s->agg_rows) s->rows_ncols = 0;
+	}
+	else if (s->kind != K_SCANROWS && s->kind != K_MOTION && s->kind != K_JOINROWS && s->kind != K_WINDOW)
+	{ exec_fail(GG_ERR_UNSUPPORTED, "WindowAgg: node kind %d below it delivers no rows", s->kind); return -1; }
+	*d = s->rows_desc;
+	return 0;
+}
+
+/* whether the plan below a WindowAgg delivers its order: a Sort whose leading keys are the partition columns, then the order
+ * columns (possibly under other WindowAggs, which keep their input's order and columns); anything without keys */
+static int window_order_ok(const GgPlan *child, const gg_window *w)
+{
+	const GgSort *so;
+	int k;
+	if (w->partNumCols + w->ordNumCols == 0) return 1;
+	while (child && child->type == T_GgWindowAgg) child = child->lefttree;
+	if (!child || child->type != T_GgSort) return 0;
+	so = (const GgSort *) child;
+	if (so->numCols < w->partNumCols + w->ordNumCols) return 0;
+	for (k = 0; k < w->partNumCols; k++) if (so->keys[k].col != w->partColIdx[k]) return 0;
+	for (k = 0; k < w->ordNumCols; k++) if (so->keys[w->partNumCols + k].col != w->ordColIdx[k]) return 0;
+	return 1;
+}
+
+/* WindowAgg (nodeWindowAgg.c ExecInitWindowAgg): checked against the device's subset and created over the child's rows; its rows
+ * are the child's columns followed by one column per function, handed up as device datum rows */
+static int init_window(GgPlanState *s, GgPlan *node, int eflags, int depth)
+{
+	GgWindowAgg *wn = (GgWindowAgg *) node;
+	const gg_window *w = &wn->win;
+	GgEState *es = s->estate;
+	gg_tupdesc in;
+	int i, a, rc;
+	s->kind = K_WINDOW;
+	if (!gg_window_create || !gg_window_run || !gg_window_free || !gg_relation_load)
+	{ exec_fail(GG_ERR_UNSUPPORTED, "WindowAgg: the device library has no window functions"); return -1; }
+	if (node->qual != -1 && (!gg_rowfilter_create || !gg_rowfilter_run || !gg_rowfilter_free))
+	{ exec_fail(GG_ERR_UNSUPPORTED, "WindowAgg with a qual: the device library has no row filter"); return -1; }
+	if (w->numFuncs < 1 || w->numFuncs > GG_MAX_WINFUNCS)
+	{ exec_fail(GG_ERR_UNSUPPORTED, "WindowAgg with %d window functions (1..%d)", w->numFuncs, GG_MAX_WINFUNCS); return -1; }
+	for (i = 0; i < w->numFuncs; i++)
+	{
+		const int32_t fn = w->funcs[i].winfnoid;
+		if (fn == GG_AGG_SUM_NUMERIC || fn == GG_AGG_AVG_NUMERIC)
+		{ exec_fail(GG_ERR_UNSUPPORTED, "WindowAgg: numeric aggregates have no device datum row"); return -1; }
+		for (a = 0; a < 3; a++)
+		{
+			const int32_t root = w->funcs[i].arg[a];
+			const gg_expr *x;
+			if (root < 0) continue;
+			if (root >= es->pool->nnodes) { exec_fail(GG_ERR_ARG, "WindowAgg: argument node %d is not in the pool", root); return -1; }
+			x = &es->pool->nodes[root];
+			if (x->kind != GG_E_VAR && x->kind != GG_E_CONST)
+			{ exec_fail(GG_ERR_UNSUPPORTED, "WindowAgg: argument %d of function %d is neither a Var nor a Const", a + 1, i + 1); return -1; }
+			if (a == 0 && is_string_type(x->rettype) && fn != GG_AGG_COUNT_ANY && (fn < GG_WF_ROW_NUMBER || fn > GG_WF_NTH_VALUE))
+			{ exec_fail(GG_ERR_UNSUPPORTED, "WindowAgg: string aggregates have no device datum row"); return -1; }
+		}
+	}
+	if (!window_order_ok(node->lefttree, w))
+	{
+		exec_fail(GG_ERR_UNSUPPORTED, "WindowAgg: the node below must be a Sort on the partition columns, then the order columns");
+		return -1;
+	}
+	if (!(s->child = init_node(node->lefttree, es, eflags, depth + 1))) return -1;
+	mark_agg_rows(s->child);
+	if (node_rows_desc(s->child, &in)) return -1;
+	if (in.natts + w->numFuncs > GG_MAX_ATTS)
+	{ exec_fail(GG_ERR_UNSUPPORTED, "WindowAgg with %d output columns (datum rows carry up to %d)", in.natts + w->numFuncs, GG_MAX_ATTS); return -1; }
+	rc = gg_window_create(es->engine, &in, w, es->pool, &s->win);
+	if (rc != GG_OK) { s->win = NULL; exec_fail(rc, "WindowAgg: %s", gg_last_error()); return -1; }
+	s->rows_desc = in;
+	for (i = 0; i < in.natts; i++) s->typid[i] = in.attrs[i].atttypid;
+	for (i = 0; i < w->numFuncs; i++)
+	{
+		gg_attr *at = &s->rows_desc.attrs[in.natts + i];
+		memset(at, 0, sizeof *at);
+		at->atttypid = w->funcs[i].wintype; at->atttypmod = -1; at->attlen = 8; at->attalign = 'd'; at->attbyval = 1;
+		s->typid[in.natts + i] = w->funcs[i].wintype;
+	}
+	s->rows_desc.natts = in.natts + w->numFuncs;
+	s->ncols = s->rows_ncols = s->rows_desc.natts;
+	s->rows_nsegs = 1;
+	if (node->qual != -1)
+	{
+		rc = gg_rowfilter_create(es->engine, &s->rows_desc, node->qual, es->pool, &s->having);
+		if (rc != GG_OK) { s->having = NULL; exec_fail(rc, "WindowAgg qual: %s", gg_last_error()); return -1; }
+	}
+	return 0;
+}
+
 static GgPlanState *init_node(GgPlan *node, GgEState *estate, int eflags, int depth)
 {
 	GgPlanState *s;
@@ -600,6 +709,11 @@ static GgPlanState *init_node(GgPlan *node, GgEState *estate, int eflags, int de
 	s = calloc(1, sizeof *s);
 	if (!s) return exec_fail(GG_ERR_NOMEM, "out of memory");
 	s->plan = node; s->estate = estate;
+	if (node->type == T_GgWindowAgg)
+	{
+		if (init_window(s, node, eflags, depth)) goto fail;
+		return s;
+	}
 	if (yields_rows(node))
 	{
 		if (node->type == T_GgHashJoin ? init_join(s, node, NULL, eflags, depth) : init_rows_node(node, estate, s)) goto fail;
@@ -707,6 +821,8 @@ static GgPlanState *init_node(GgPlan *node, GgEState *estate, int eflags, int de
 		case T_GgHash:
 			s->kind = K_HASH;          /* marker: the build is part of the join's pipeline */
 			return s;
+		case T_GgWindowAgg:
+			break;                     /* handled above */
 	}
 	exec_fail(GG_ERR_UNSUPPORTED, "unknown node type %d", (int) node->type);
 fail:
@@ -906,6 +1022,7 @@ static int sort_host_rows(GgPlanState *s, const GgPlanState *src, const gg_sortk
 }
 
 static int run_node(GgPlanState *s);
+static int ensure_rows(GgPlanState *s);
 
 static int run_child(GgPlanState *s)
 {
@@ -998,7 +1115,7 @@ static int run_rows_node(GgPlanState *s)
 /* the device buffer that holds a rows node's datum rows */
 static gg_relation *rows_buffer(const GgPlanState *s)
 {
-	if (s->kind == K_JOINROWS || s->agg_rows) return s->rows_rel;        /* the join's / the Agg's own output buffer */
+	if (s->kind == K_JOINROWS || s->kind == K_WINDOW || s->agg_rows) return s->rows_rel;   /* the join's / window's / Agg's own output */
 	return s->rows_recv && s->rows_nsegs > 1 ? s->rows_recv : s->rows_send;
 }
 
@@ -1072,36 +1189,75 @@ static int agg_datumrows(GgPlanState *s)
 	return hand_up_rows(s, out);
 }
 
+/* the host rows of src uploaded once as datum rows into s->rows_send; *view wraps them (the caller frees it) */
+static int upload_host_rows(GgPlanState *s, const GgPlanState *src, gg_relation **view)
+{
+	GgEState *es = s->estate;
+	const uint64_t n = src->nrows > 0 ? (uint64_t) src->nrows : 0, W = 1 + (uint64_t) src->ncols;
+	const uint64_t nb = (n * W * 8 + 16 + GG_BLCKSZ - 1) / GG_BLCKSZ;
+	uint64_t *buf, r;
+	int c, rc;
+	*view = NULL;
+	if (s->rows_send && gg_relation_nblocks(s->rows_send) < nb) { gg_relation_free(s->rows_send); s->rows_send = NULL; }
+	if (!s->rows_send && (rc = gg_relation_create(es->engine, nb, &s->rows_send)) != GG_OK)
+	{ s->rows_send = NULL; exec_fail(rc, "rows: %s", gg_last_error()); return -1; }
+	buf = calloc((size_t) nb, GG_BLCKSZ);
+	if (!buf) { exec_fail(GG_ERR_NOMEM, "out of memory"); return -1; }
+	for (r = 0; r < n; r++)
+		for (c = 0; c < src->ncols; c++)
+		{
+			buf[r * W] |= (uint64_t) (src->isnull[r * (uint64_t) src->ncols + c] != 0) << c;
+			buf[r * W + 1 + c] = (uint64_t) src->values[r * (uint64_t) src->ncols + c];
+		}
+	rc = gg_relation_load(s->rows_send, 0, buf, nb);              /* pageable: staged before the call returns, so buf can go */
+	free(buf);
+	if (rc == GG_OK) rc = gg_relation_attach_rows(es->engine, gg_relation_device_ptr(s->rows_send), n, src->ncols, view);
+	if (rc != GG_OK) { *view = NULL; exec_fail(rc, "rows: %s", gg_last_error()); return -1; }
+	return 0;
+}
+
 /* A FINAL Agg whose groups were finalised on the host (its child delivered host rows, or the slice was re-run with host-row
  * Motions), under a HAVING filter or a HashJoin: its host rows uploaded once as datum rows (into rows_send) and handed up as the
  * device path hands them up, so the qual is evaluated one way only */
 static int upload_agg_rows(GgPlanState *s)
 {
-	GgEState *es = s->estate;
-	const uint64_t n = s->nrows > 0 ? (uint64_t) s->nrows : 0, W = 1 + (uint64_t) s->ncols;
-	const uint64_t nb = (n * W * 8 + 16 + GG_BLCKSZ - 1) / GG_BLCKSZ;
 	gg_relation *view = NULL;
-	uint64_t *buf, r;
-	int c, rc;
-	if (s->rows_send && gg_relation_nblocks(s->rows_send) < nb) { gg_relation_free(s->rows_send); s->rows_send = NULL; }
-	if (!s->rows_send && (rc = gg_relation_create(es->engine, nb, &s->rows_send)) != GG_OK)
-	{ s->rows_send = NULL; exec_fail(rc, "Agg rows: %s", gg_last_error()); return -1; }
-	buf = calloc((size_t) nb, GG_BLCKSZ);
-	if (!buf) { exec_fail(GG_ERR_NOMEM, "out of memory"); return -1; }
-	for (r = 0; r < n; r++)
-		for (c = 0; c < s->ncols; c++)
-		{
-			buf[r * W] |= (uint64_t) (s->isnull[r * (uint64_t) s->ncols + c] != 0) << c;
-			buf[r * W + 1 + c] = (uint64_t) s->values[r * (uint64_t) s->ncols + c];
-		}
-	rc = gg_relation_load(s->rows_send, 0, buf, nb);              /* pageable: staged before the call returns, so buf can go */
-	free(buf);
-	if (rc == GG_OK) rc = gg_relation_attach_rows(es->engine, gg_relation_device_ptr(s->rows_send), n, s->ncols, &view);
-	if (rc != GG_OK) { exec_fail(rc, "Agg rows: %s", gg_last_error()); return -1; }
-	s->rows_n = n;
+	int rc;
+	if (upload_host_rows(s, s, &view)) return -1;
+	s->rows_n = s->nrows > 0 ? (uint64_t) s->nrows : 0;
 	rc = hand_up_rows(s, view);
 	gg_relation_free(view);
 	return rc;
+}
+
+/* WindowAgg: the child's sorted rows windowed where they are (or, when they ended up on the host, uploaded once), then through
+ * the qual when there is one; the result stays on the device for the node above */
+static int run_window(GgPlanState *s)
+{
+	GgEState *es = s->estate;
+	GgPlanState *ch = s->child;
+	gg_relation *in = NULL, *up = NULL, *out = NULL;
+	uint64_t nin, nout = 0;
+	int rc;
+	drop_device_results(s);
+	if (run_child(s)) return -1;
+	s->nonreceiver = ch->nonreceiver;
+	if (ch->rows_rel && !ch->rows_ready) { in = ch->rows_rel; nin = ch->rows_n; }
+	else
+	{
+		if (ensure_rows(ch) || upload_host_rows(s, ch, &up)) return -1;
+		in = up; nin = ch->nrows > 0 ? (uint64_t) ch->nrows : 0;
+	}
+	rc = gg_window_run(s->win, in, nin, &out, &nout);
+	s->win_ms = 0.0f;
+	if (rc == GG_OK && gg_engine_last_kernel_ms) (void) gg_engine_last_kernel_ms(es->engine, &s->win_ms);
+	if (rc == GG_OK && s->having) rc = gg_rowfilter_run(s->having, out, nout, &out, &nout);
+	if (rc == GG_OK) rc = gg_relation_attach_rows(es->engine, gg_relation_device_ptr(out), nout, s->rows_ncols, &s->rows_rel);
+	if (up) gg_relation_free(up);
+	if (rc != GG_OK) { s->rows_rel = NULL; exec_fail(rc, "%s", gg_last_error()); return -1; }
+	s->rows_n = nout;
+	s->rows_ready = 0;
+	return 0;
 }
 
 /* a node's aggregate rows -> host result arrays, from its device group records (the one synchronisation of a
@@ -1581,6 +1737,7 @@ static int run_node(GgPlanState *s)
 		case K_SORT: rc = run_sort(s); break;
 		case K_MOTION: rc = run_motion(s); break;
 		case K_LIMIT: rc = run_limit(s); break;
+		case K_WINDOW: rc = run_window(s); break;
 		default:
 			exec_fail(GG_ERR_ARG, "bad plan state");
 			return -1;
@@ -1666,6 +1823,7 @@ int GgExecNodeInstrumentation(GgPlanState *s, GgInstrumentation *out)
 	if ((s->kind == K_JOINAGG || s->kind == K_JOINROWS) && s->ja) out->hash_batches = gg_joinagg_nbatch(s->ja);
 	if ((s->kind == K_SCANAGG && s->sa) || ((s->kind == K_JOINAGG || s->kind == K_JOINROWS) && s->ja))
 		if (GgExecPipelineKernelMs(s, &ms, &launches, &variant, &bms) == GG_OK) out->kernel_ms = ms + bms;
+	if (s->kind == K_WINDOW) out->kernel_ms = s->win_ms;
 	return GG_OK;
 }
 
@@ -1953,6 +2111,12 @@ void GgExecSquelchLimit(GgPlanState *node) { GgExecSquelchNode(node); }
 /* ExecSortMarkPos / ExecSortRestrPos (nodeSort.c:444,462): the sorted result is materialised, so a position is an index */
 void GgExecSortMarkPos(GgPlanState *node) { if (node && node->done) node->markpos = node->next; }
 void GgExecSortRestrPos(GgPlanState *node) { if (node && node->done) node->next = node->markpos; }
+
+GgPlanState *GgExecInitWindowAgg(GgWindowAgg *node, GgEState *estate, int eflags) { return init_tagged(&node->plan, T_GgWindowAgg, estate, eflags); }
+GgTupleTableSlot *GgExecWindowAgg(GgPlanState *node) { return GgExecProcNode(node); }
+void GgExecEndWindowAgg(GgPlanState *node) { GgExecEndNode(node); }
+int GgExecReScanWindowAgg(GgPlanState *node) { return GgExecReScan(node); }
+void GgExecSquelchWindowAgg(GgPlanState *node) { GgExecSquelchNode(node); }
 
 GgPlanState *GgExecInitMotion(GgMotion *node, GgEState *estate, int eflags) { return init_tagged(&node->plan, T_GgMotion, estate, eflags); }
 GgTupleTableSlot *GgExecMotion(GgPlanState *node) { return GgExecProcNode(node); }

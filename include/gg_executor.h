@@ -7,7 +7,7 @@
  *     ExecEndNode    src/backend/executor/execProcnode.c:1315
  *     ExecReScan     src/backend/executor/execAmi.c:76
  *     ExecSquelchNode src/backend/executor/execAmi.c:641
- * with the node types of the accelerated path (plannodes.h): SeqScan, Agg, Hash, HashJoin, Sort, Motion, Limit.
+ * with the node types of the accelerated path (plannodes.h): SeqScan, Agg, Hash, HashJoin, Sort, Motion, Limit, WindowAgg.
  * Names keep the reference's, prefixed Gg.  The plan tree is what the Postgres-side translator of
  * INTEGRATION.md §2 builds from the real Plan tree; expressions live in one gg_exprpool.
  *
@@ -21,6 +21,9 @@
  *     Agg with HAVING (plan.qual)             its groups as device datum rows, filtered on the device (gg_rowfilter_run);
  *                                             refused (GG_ERR_UNSUPPORTED) where that cannot run, never run without its qual
  *     HashJoin <- Agg (either side)           the Agg's groups as device datum rows, scanned by the join like join rows
+ *     WindowAgg <- Sort <- any row producer  the sorted rows windowed on the device (gg_window_run), its optional qual (a
+ *                                             SubqueryScan's, e.g. rn <= 3) by gg_rowfilter_run; device datum rows for the
+ *                                             caller, a Limit, a Sort, another WindowAgg, an Agg, a HashJoin or a Motion
  *     Motion <- any of the above              rows handed to the transport  (GgMotionTransport)
  * and returns NULL with GgExecLastError() set when a node or a shape is outside the accelerated subset, so the
  * caller keeps the CPU nodes for that subtree (there is no CPU implementation behind this API).
@@ -42,7 +45,8 @@ typedef enum GgNodeTag {            /* nodes/nodes.h NodeTag, the accelerated su
 	T_GgHashJoin,
 	T_GgSort,
 	T_GgMotion,
-	T_GgLimit
+	T_GgLimit,
+	T_GgWindowAgg
 } GgNodeTag;
 
 typedef enum GgMotionType {         /* plannodes.h MotionType */
@@ -122,6 +126,18 @@ typedef struct GgLimit {
 	int64_t limitOffset, limitCount;
 } GgLimit;
 
+/* WindowAgg (plannodes.h:1145): the child's rows, each followed by one column per window function (gg_plan.h gg_window).  The
+ * child must deliver the window's order: a Sort whose leading keys are the partition columns, then the order columns (or a
+ * WindowAgg over such a Sort); with neither partition nor order columns any row producer will do.  plan.qual (-1 = none) is a
+ * qual over the output row, Vars varno 0 with 1-based varattno: what a translator folds in from a trivial SubqueryScan above.
+ * Refused (GG_ERR_UNSUPPORTED) where the device cannot run it: value-offset frames, numeric aggregates, an argument that is
+ * neither a Var nor a Const, more than GG_MAX_WINFUNCS functions or GG_MAX_ATTS output columns, an input in the wrong order, a
+ * device library without gg_window_*. */
+typedef struct GgWindowAgg {
+	GgPlan plan;
+	gg_window win;
+} GgWindowAgg;
+
 /* TupleTableSlot holding a virtual tuple (tuptable.h:117-175): Datums + null flags */
 typedef struct GgTupleTableSlot {
 	int32_t  tts_nvalid;
@@ -191,7 +207,7 @@ void GgExecSquelchNode(GgPlanState *node);
 const char *GgExecLastError(void);
 int  GgExecLastErrorCode(void);                /* GG_ERR_* of the failure, GG_OK if none */
 /* introspection: which device pipeline a state node was fused into ("scanagg", "joinagg", "joinrows", "sort", "motion",
- * "limit", ...) */
+ * "limit", "windowagg", ...) */
 const char *GgExecNodeKind(GgPlanState *node);
 /* where a node that has run keeps its result: "device-groups" (aggregate rows as group records), "device-rows" (datum rows)
  * or "host" (Datum arrays); "" before it has run */
@@ -248,6 +264,12 @@ GgTupleTableSlot *GgExecLimit(GgPlanState *node);
 void GgExecEndLimit(GgPlanState *node);
 int  GgExecReScanLimit(GgPlanState *node);
 void GgExecSquelchLimit(GgPlanState *node);
+/* nodeWindowAgg.h */
+GgPlanState *GgExecInitWindowAgg(GgWindowAgg *node, GgEState *estate, int eflags);
+GgTupleTableSlot *GgExecWindowAgg(GgPlanState *node);
+void GgExecEndWindowAgg(GgPlanState *node);
+int  GgExecReScanWindowAgg(GgPlanState *node);
+void GgExecSquelchWindowAgg(GgPlanState *node);
 void GgExecSortMarkPos(GgPlanState *node);      /* nodeSort.c:444 ExecSortMarkPos */
 void GgExecSortRestrPos(GgPlanState *node);     /* nodeSort.c:462 ExecSortRestrPos */
 GgPlanState *GgExecInitHashJoin(GgHashJoin *node, GgEState *estate, int eflags);

@@ -309,6 +309,60 @@ typedef struct gg_sortkey {         /* Sort.sortColIdx/sortOperators/nullsFirst 
 	int32_t nulls_first;
 } gg_sortkey;
 
+/* ---- window functions (WindowAgg, plannodes.h:1145; WindowFunc, primnodes.h) ---- */
+/* frame_clause options (parsenodes.h:495-517) */
+#define GG_FRAMEOPTION_NONDEFAULT                0x00001
+#define GG_FRAMEOPTION_RANGE                     0x00002
+#define GG_FRAMEOPTION_ROWS                      0x00004
+#define GG_FRAMEOPTION_BETWEEN                   0x00008
+#define GG_FRAMEOPTION_START_UNBOUNDED_PRECEDING 0x00010
+#define GG_FRAMEOPTION_END_UNBOUNDED_PRECEDING   0x00020
+#define GG_FRAMEOPTION_START_UNBOUNDED_FOLLOWING 0x00040
+#define GG_FRAMEOPTION_END_UNBOUNDED_FOLLOWING   0x00080
+#define GG_FRAMEOPTION_START_CURRENT_ROW         0x00100
+#define GG_FRAMEOPTION_END_CURRENT_ROW           0x00200
+#define GG_FRAMEOPTION_START_VALUE_PRECEDING     0x00400
+#define GG_FRAMEOPTION_END_VALUE_PRECEDING       0x00800
+#define GG_FRAMEOPTION_START_VALUE_FOLLOWING     0x01000
+#define GG_FRAMEOPTION_END_VALUE_FOLLOWING       0x02000
+#define GG_FRAMEOPTION_DEFAULTS (GG_FRAMEOPTION_RANGE | GG_FRAMEOPTION_START_UNBOUNDED_PRECEDING | GG_FRAMEOPTION_END_CURRENT_ROW)
+
+/* window function OIDs (pg_proc.h:4874-4902); the aggregates allowed as window functions are the GG_AGG_* above, numeric excepted */
+#define GG_WF_ROW_NUMBER        3100   /* int8 */
+#define GG_WF_RANK              3101   /* int8 */
+#define GG_WF_DENSE_RANK        3102   /* int8 */
+#define GG_WF_PERCENT_RANK      3103   /* float8 */
+#define GG_WF_CUME_DIST         3104   /* float8 */
+#define GG_WF_NTILE             3105   /* int4; ntile(n), n a Const */
+#define GG_WF_LAG               3106   /* lag(x) */
+#define GG_WF_LAG_OFFSET        3107   /* lag(x, int4 offset) */
+#define GG_WF_LAG_DEFAULT       3108   /* lag(x, int4 offset, default) */
+#define GG_WF_LEAD              3109
+#define GG_WF_LEAD_OFFSET       3110
+#define GG_WF_LEAD_DEFAULT      3111
+#define GG_WF_FIRST_VALUE       3112
+#define GG_WF_LAST_VALUE        3113
+#define GG_WF_NTH_VALUE         3114   /* nth_value(x, n), n a Const */
+
+#define GG_MAX_WINFUNCS 8
+
+typedef struct gg_winfunc {         /* WindowFunc (primnodes.h) */
+	int32_t winfnoid;                   /* GG_WF_* or GG_AGG_* */
+	int32_t wintype;                    /* type OID of the result */
+	int32_t arg[3];                     /* expression roots in the pool, -1 = absent: a Var of the input row (varno 0) or a Const */
+	int32_t pad;
+} gg_winfunc;
+
+typedef struct gg_window {          /* WindowAgg (plannodes.h:1145) */
+	int32_t partNumCols;
+	int32_t partColIdx[GG_MAX_KEYS];    /* 0-based columns of the input rows */
+	int32_t ordNumCols;
+	int32_t ordColIdx[GG_MAX_KEYS];
+	int32_t frameOptions;               /* GG_FRAMEOPTION_* */
+	int32_t numFuncs;
+	gg_winfunc funcs[GG_MAX_WINFUNCS];
+} gg_window;
+
 enum gg_motiontype {                /* plannodes.h MotionType */
 	GG_MOTION_HASH = 0,                 /* Redistribute */
 	GG_MOTION_FIXED = 1,                /* Broadcast / Gather */

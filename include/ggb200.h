@@ -280,6 +280,25 @@ void gg_rowfilter_free(gg_rowfilter *f);
 void gg_groups_set_nonreceiver(gg_groups *g);
 void gg_groups_free(gg_groups *g);
 
+/* ---- WindowAgg over datum rows (nodeWindowAgg.c, utils/adt/windowfuncs.c) ----
+ * rows_desc is the GG_FMT_DATUMROWS descriptor of the input rows, which arrive sorted so that partitions (equal partition
+ * columns) and peer groups (equal order columns within a partition) are runs: the planner's Sort below a WindowAgg.  Equality is
+ * execTuplesMatch's: two NULLs match, float8 -0 = +0 and NaN = NaN, packed strings compare by bits.  win describes the node
+ * (gg_plan.h gg_window); each function's arguments are Vars of the input row (varno 0, 1-based varattno) or Consts.
+ * create checks the plan: GG_ERR_UNSUPPORTED with a message for a frame with value offsets, a numeric or unknown function, an
+ * argument that is neither a Var nor a Const, a non-Const ntile / nth_value argument, or more than GG_MAX_ATTS output columns;
+ * GG_ERR_ARG for a column or a root out of range.
+ * run windows the first nrows slots of a datum-row relation of rows_desc's columns: *out_view receives one row per live input
+ * row, in input order, of the input's columns followed by one column per function (word 0: the NULL mask over all of them);
+ * dead slots (GG_DATUMROW_DEAD) get no number and no output row.  The view is owned by the window object, valid until its next
+ * run or free.  nrows == 0 launches nothing.  Errors: GG_ERR_WINDOW_ARG for ntile / nth_value of a Const <= 0 over at least one
+ * row (the reference's message), GG_ERR_FLOAT_OVERFLOW for a float8 sum / avg that becomes infinite with no infinite input. */
+typedef struct gg_window_obj gg_window_obj;
+#define GG_ERR_WINDOW_ARG      (-14)   /* "argument of ntile / nth_value must be greater than zero", SQLSTATE 22014 / 22016 */
+int  gg_window_create(gg_engine *e, const gg_tupdesc *rows_desc, const gg_window *win, const gg_exprpool *pool, gg_window_obj **out);
+int  gg_window_run(gg_window_obj *w, gg_relation *rows, uint64_t nrows, gg_relation **out_view, uint64_t *nout);
+void gg_window_free(gg_window_obj *w);
+
 /* ---- Interconnect: the Motion layer over NCCL ----
  * Replaces SetupInterconnect / TeardownInterconnect and the ChunkTransportState vtable of the UDP interconnect
  * (cdb/cdbinterconnect.h:500-533, cdb/motion/ic_common.c:522,560, cdbmotion.c:434,559) for GPU segments: one NCCL
