@@ -606,10 +606,10 @@ static int init_having(GgPlanState *s, int32_t qual)
 static int node_rows_desc(GgPlanState *s, gg_tupdesc *d)
 {
 	if (s->kind == K_SORT || s->kind == K_LIMIT || (s->kind == K_MOTION && !s->rows_scan)) return node_rows_desc(s->child, d);
-	if ((s->kind == K_SCANAGG || s->kind == K_JOINAGG || s->kind == K_AGGFINAL) && !s->having)
+	if (s->kind == K_SCANAGG || s->kind == K_JOINAGG || s->kind == K_AGGFINAL)
 	{
 		/* the descriptor of its output columns (a HAVING's init made it already); an Agg that hands up host rows keeps no row width */
-		if (agg_rows_desc(s)) return -1;
+		if (!s->having && agg_rows_desc(s)) return -1;
 		if (!s->agg_rows) s->rows_ncols = 0;
 	}
 	else if (s->kind != K_SCANROWS && s->kind != K_MOTION && s->kind != K_JOINROWS && s->kind != K_WINDOW)
