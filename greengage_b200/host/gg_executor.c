@@ -57,6 +57,21 @@ enum { K_SCANAGG = 1, K_JOINAGG, K_AGGFINAL, K_SORT, K_MOTION, K_SCANROWS, K_HAS
 #pragma weak gg_window_free
 #pragma weak gg_engine_last_kernel_ms
 
+/* what the device library offers, one group of the entry points above each.  gg_relation_load is older than the aggregate datum
+ * rows and the window functions, so a library with either can also upload host rows to them. */
+static int lib_has_bounded_sort(void) { return gg_sort_rows_bounded && gg_sort_datumrows_bounded; }
+static int lib_has_join_rows(void) { return gg_joinrows_create && gg_joinagg_rows; }
+static int lib_has_agg_rows(void) { return gg_scanagg_datumrows && gg_joinagg_datumrows && gg_groups_datumrows && gg_relation_load; }
+static int lib_has_rowfilter(void) { return gg_rowfilter_create && gg_rowfilter_run && gg_rowfilter_free; }
+static int lib_has_window(void) { return gg_window_create && gg_window_run && gg_window_free && gg_relation_load; }
+
+/* what the node above reads of a node, said to init_node: host rows; device datum rows where the node can give them (a Sort, a
+ * Limit or a WindowAgg, which also take host rows); or device datum rows only (a HashJoin input, refused otherwise) */
+enum { WANT_HOST, WANT_ROWS, WANT_ROWS_ONLY };
+
+/* where a node that has run keeps the result it hands up */
+enum { R_NONE, R_GROUPS, R_ROWS, R_HOST };
+
 struct GgPlanState {
 	int kind;
 	GgPlan *plan;
@@ -73,15 +88,15 @@ struct GgPlanState {
 	uint64_t host_nblocks;
 	gg_agg agg;
 	/* device-resident results */
-	gg_groups *groups;                  /* aggregate rows */
+	gg_groups *groups;                  /* group records available to a Motion or FINAL Agg above (also when the result is on the
+	                                     * host: aggrows_to_host runs first, then pipeline_groups) */
 	gg_relation *rows_rel;              /* datum rows (K_SCANROWS, K_MOTION over a scan): wraps rows_recv / rows_send; K_JOINROWS:
 	                                     * wraps the join's output */
 	gg_relation *rows_send, *rows_recv; /* raw device buffers (gg_relation_create) */
 	uint64_t rows_cap;                  /* rows the send buffer holds over all destinations */
 	uint64_t rows_n;
-	int32_t rows_ncols;
 	int32_t rows_targets[GG_MAX_OUTCOLS];
-	gg_tupdesc rows_desc;               /* GG_FMT_DATUMROWS descriptor of what this node delivers */
+	gg_tupdesc rows_desc;               /* GG_FMT_DATUMROWS descriptor of what this node delivers; natts: the rows' width */
 	GgSeqScan *rows_scan;               /* the SeqScan the rows come from */
 	int32_t rows_nsegs;                 /* destinations the rows are partitioned for (1: plain projection) */
 	/* result set: filled on demand, then handed out row by row */
@@ -89,19 +104,18 @@ struct GgPlanState {
 	int sort_runs;                      /* Sort over host rows: sorted runs the last execution merged (1: it fitted the operator's memory) */
 	uint64_t sort_bound;                /* Sort: rows the Limit above wants (SortState.bound, set by pass_down_bound); GG_NO_BOUND: all */
 	double instr_ntuples, instr_nloops; /* Instrumentation: tuples handed up, executions */
-	int rows_ready;                     /* host arrays below are filled */
+	int result;                         /* R_*: read from groups, rows_rel or the host arrays below */
 	int squelched;
 	int nonreceiver;                    /* above a Gather, on a segment that is not its receiver: no rows at all */
 	int dev_groups;                     /* decided at init, from the plan alone (so every segment decides alike): this node hands
 	                                     * its aggregate rows up as device-resident group records */
-	int agg_rows;                       /* decided at init, from the plan alone: an Agg directly under a Sort or a Limit, under a
-	                                     * HashJoin, or with a HAVING qual hands up its groups finalised into device datum rows
-	                                     * (rows_rel), which the node above sorts, windows or joins where they are */
+	int agg_rows;                       /* decided at the end of an Agg's init, from the plan alone: WANT_ROWS hands up the groups
+	                                     * finalised on the device as device datum rows (rows_rel), which the node above sorts or
+	                                     * windows where they are; WANT_ROWS_ONLY (a HAVING qual, or a HashJoin above) also uploads
+	                                     * groups a FINAL Agg finalised on the host; WANT_HOST: host rows */
 	gg_rowfilter *having;               /* an Agg's plan.qual (HAVING), compiled at init over its rows_desc; a WindowAgg's qual */
 	gg_window_obj *win;                 /* K_WINDOW: the window functions, created at init over the child's rows */
 	float win_ms;                       /* K_WINDOW: CUDA-event time of the last gg_window_run */
-	int rows_required;                  /* an Agg under a HashJoin: the join reads device rows only, so a FINAL Agg whose groups were
-	                                     * finalised on the host uploads them */
 	int lazy_fetch;                     /* set by a Motion above that moves this node's records on the device: the pipeline's result
 	                                     * is not fetched to the host before it travels (no host synchronisation between the scan
 	                                     * and the Motion); what a fetch would have decided travels as status flags */
@@ -157,8 +171,8 @@ const char *GgExecNodeKind(GgPlanState *s)
 const char *GgExecNodeResultLocation(GgPlanState *s)
 {
 	if (!s || !s->done) return "";
-	if (s->rows_rel && !s->rows_ready) return "device-rows";
-	if (s->groups && !s->rows_ready) return "device-groups";
+	if (s->result == R_ROWS) return "device-rows";
+	if (s->result == R_GROUPS) return "device-groups";
 	return "host";
 }
 
@@ -288,7 +302,7 @@ static int rows_from_aggrows(GgPlanState *s, const gg_aggrow *rows, int n)
 			c += w;
 		}
 	}
-	s->rows_ready = 1;
+	s->result = R_HOST;
 	return 0;
 }
 
@@ -332,6 +346,7 @@ static void drop_device_results(GgPlanState *s)
 {
 	if (s->groups) { gg_groups_free(s->groups); s->groups = NULL; }
 	if (s->rows_rel) { gg_relation_free(s->rows_rel); s->rows_rel = NULL; }
+	s->result = R_NONE;
 }
 
 static void end_tree(GgPlanState *s)
@@ -352,13 +367,13 @@ static void end_tree(GgPlanState *s)
 
 #define GG_MAX_PLAN_DEPTH 32        /* the deepest accelerated slice is Motion <- Sort <- Agg <- Motion <- Agg <- HashJoin <- Hash <- Motion <- SeqScan */
 
-static GgPlanState *init_node(GgPlan *node, GgEState *estate, int eflags, int depth);
+static GgPlanState *init_node(GgPlan *node, GgEState *estate, int eflags, int depth, int want);
 
 GgPlanState *GgExecInitNode(GgPlan *node, GgEState *estate, int eflags)
 {
 	g_err[0] = 0; g_errcode = GG_OK;
 	g_local_code = 0; g_local_err[0] = 0;
-	return init_node(node, estate, eflags, 0);
+	return init_node(node, estate, eflags, 0, WANT_HOST);
 }
 
 static int multi_segment(const GgEState *es) { return es->nsegs > 1; }
@@ -393,32 +408,13 @@ static int is_pipeline_input(const GgPlan *p) { return p && (p->type == T_GgSeqS
 /* a join also reads the groups of an Agg, finalised into device datum rows (init_input checks that it can deliver them) */
 static int is_join_input(const GgPlan *p) { return is_pipeline_input(p) || (p && p->type == T_GgAgg); }
 
-static void mark_agg_rows(GgPlanState *ch);
-static int agg_rows_desc(GgPlanState *s);
-
 static int init_input(GgPlanState *s, GgPlan *p, int eflags, int depth, gg_scan *scan, GgPlanState **rows, gg_relation **rel)
 {
 	memset(scan, 0, sizeof *scan);
-	if (p->type == T_GgAgg)
+	if (yields_rows(p) || p->type == T_GgAgg)
 	{
-		/* an Agg under a HashJoin hands up its groups as device rows, by the rule of an Agg under a Sort (mark_agg_rows) */
-		GgPlanState *ch;
-		if (!(ch = *rows = init_node(p, s->estate, eflags, depth))) return -1;
-		mark_agg_rows(ch);
-		if (!ch->agg_rows || !gg_relation_load)
-		{
-			exec_fail(GG_ERR_UNSUPPORTED, "HashJoin over an Agg: only a one-stage Agg over a scan or a join, or a FINAL Agg over device "
-			          "group records, without numeric aggregates, delivers its groups as device rows");
-			return -1;
-		}
-		if (!ch->having && agg_rows_desc(ch)) return -1;
-		ch->rows_required = 1;
-		scan->desc = ch->rows_desc; scan->qual = -1;
-		return 0;
-	}
-	if (yields_rows(p))
-	{
-		if (!(*rows = init_node(p, s->estate, eflags, depth))) return -1;
+		/* a join reads device rows only: an Agg that cannot finalise its groups into them is refused at its init */
+		if (!(*rows = init_node(p, s->estate, eflags, depth, WANT_ROWS_ONLY))) return -1;
 		scan->desc = (*rows)->rows_desc; scan->qual = -1;
 		return 0;
 	}
@@ -426,35 +422,50 @@ static int init_input(GgPlanState *s, GgPlan *p, int eflags, int depth, gg_scan 
 	return bind_relation(s->estate, (GgSeqScan *) p, rel, &s->host_pages, &s->host_nblocks);
 }
 
+/* s hands up datum rows of `ncols` columns of these types, each an 8-byte word (GG_FMT_DATUMROWS): its row descriptor, typid[]
+ * and ncols.  notnull[c] (NULL: none) where the producer is certain column c is never NULL: a wrong NOT NULL would select a
+ * consumer's NULL-free kernel variant over NULLs. */
+static void set_rows_layout(GgPlanState *s, int ncols, const int32_t *types, const int8_t *notnull)
+{
+	int c;
+	memset(&s->rows_desc, 0, sizeof s->rows_desc);
+	s->rows_desc.natts = ncols;
+	s->rows_desc.format = GG_FMT_DATUMROWS;
+	for (c = 0; c < ncols; c++)
+	{
+		gg_attr *a = &s->rows_desc.attrs[c];
+		a->atttypid = types[c]; a->atttypmod = -1; a->attlen = 8; a->attalign = 'd'; a->attbyval = 1;
+		a->attnotnull = notnull ? notnull[c] : 0;
+		s->typid[c] = types[c];
+	}
+	s->ncols = ncols;
+}
+
 /* state of a rows-producing node (SeqScan with targets, optionally under a Redistribute Motion) */
 static int init_rows_node(GgPlan *node, GgEState *estate, GgPlanState *s)
 {
 	GgSeqScan *sc = (GgSeqScan *) (node->type == T_GgMotion ? node->lefttree : node);
 	const void *hp; uint64_t hn;
+	int32_t types[GG_MAX_OUTCOLS];
+	int8_t notnull[GG_MAX_OUTCOLS];
 	int i;
 	if (sc->numTargets < 1 || sc->numTargets > GG_MAX_OUTCOLS || sc->numTargets > 16)
 	{ exec_fail(GG_ERR_UNSUPPORTED, "SeqScan projecting %d columns (1..16 travel as datum rows)", sc->numTargets); return -1; }
 	if (bind_relation(estate, sc, &s->rel, &hp, &hn)) return -1;
 	if (!s->rel) { exec_fail(GG_ERR_UNSUPPORTED, "a row-producing SeqScan needs its relation resident on the device"); return -1; }
 	s->rows_scan = sc;
-	s->rows_ncols = sc->numTargets;
-	memset(&s->rows_desc, 0, sizeof s->rows_desc);
-	s->rows_desc.natts = sc->numTargets;
-	s->rows_desc.format = GG_FMT_DATUMROWS;
 	for (i = 0; i < sc->numTargets; i++)
 	{
 		const int32_t root = sc->targets[i];
 		const gg_expr *e;
-		gg_attr *a = &s->rows_desc.attrs[i];
 		if (root < 0 || root >= estate->pool->nnodes) { exec_fail(GG_ERR_ARG, "SeqScan target %d: node %d is not in the pool", i, root); return -1; }
 		e = &estate->pool->nodes[root];
 		s->rows_targets[i] = root;
-		s->typid[i] = e->rettype;
-		a->atttypid = e->rettype; a->atttypmod = -1; a->attlen = 8; a->attalign = 'd'; a->attbyval = 1;
+		types[i] = e->rettype;
 		/* a plain Var of a NOT NULL column stays NOT NULL: lets the consumers run their NULL-free kernel variants */
-		a->attnotnull = (e->kind == 1 /* GG_E_VAR */ && e->varattno >= 1 && e->varattno <= sc->desc.natts) ? sc->desc.attrs[e->varattno - 1].attnotnull : 0;
+		notnull[i] = (e->kind == 1 /* GG_E_VAR */ && e->varattno >= 1 && e->varattno <= sc->desc.natts) ? sc->desc.attrs[e->varattno - 1].attnotnull : 0;
 	}
-	s->ncols = sc->numTargets;
+	set_rows_layout(s, sc->numTargets, types, notnull);
 	if (node->type == T_GgMotion)
 	{
 		GgMotion *mo = (GgMotion *) node;
@@ -486,8 +497,10 @@ static int init_join(GgPlanState *s, GgPlan *node, const gg_agg *agg, int eflags
 	GgHashJoin *hj = (GgHashJoin *) node;
 	GgPlan *outer = node->lefttree, *hash = node->righttree, *inner = hash ? hash->lefttree : NULL;
 	gg_scan oscan, iscan;
+	int32_t types[GG_MAX_OUTCOLS];
+	int8_t notnull[GG_MAX_OUTCOLS];
 	int rc, i;
-	if (!agg && (!gg_joinrows_create || !gg_joinagg_rows))
+	if (!agg && !lib_has_join_rows())
 	{ exec_fail(GG_ERR_UNSUPPORTED, "HashJoin with a target list: the device library has no join that writes its rows"); return -1; }
 	if (!agg && (hj->numTargets > GG_MAX_OUTCOLS || hj->numTargets > 16))
 	{ exec_fail(GG_ERR_UNSUPPORTED, "HashJoin projecting %d columns (1..16 travel as datum rows)", hj->numTargets); return -1; }
@@ -513,24 +526,17 @@ static int init_join(GgPlanState *s, GgPlan *node, const gg_agg *agg, int eflags
 	if (rc != GG_OK) { exec_fail(rc, "HashJoin: %s", gg_last_error()); return -1; }
 	/* the rows' descriptor: a column of the side a join null-extends is nullable; a plain Var of a NOT NULL column of the other
 	 * side stays NOT NULL, as a scan's projection keeps it */
-	s->rows_ncols = hj->numTargets;
-	s->rows_nsegs = 1;
-	s->ncols = hj->numTargets;
-	memset(&s->rows_desc, 0, sizeof s->rows_desc);
-	s->rows_desc.natts = hj->numTargets;
-	s->rows_desc.format = GG_FMT_DATUMROWS;
 	for (i = 0; i < hj->numTargets; i++)
 	{
 		const gg_expr *e = &estate->pool->nodes[hj->targets[i]];          /* checked by gg_joinrows_create */
 		const int jt = hj->hj.jointype;
 		const int nullext = e->varno == 0 ? (jt == GG_JOIN_RIGHT || jt == GG_JOIN_FULL) : (jt == GG_JOIN_LEFT || jt == GG_JOIN_FULL);
 		const gg_tupdesc *d = e->varno == 0 ? &oscan.desc : &iscan.desc;
-		gg_attr *a = &s->rows_desc.attrs[i];
 		s->rows_targets[i] = hj->targets[i];
-		s->typid[i] = e->rettype;
-		a->atttypid = e->rettype; a->atttypmod = -1; a->attlen = 8; a->attalign = 'd'; a->attbyval = 1;
-		a->attnotnull = (e->kind == 1 /* GG_E_VAR */ && !nullext && e->varattno >= 1 && e->varattno <= d->natts) ? d->attrs[e->varattno - 1].attnotnull : 0;
+		types[i] = e->rettype;
+		notnull[i] = (e->kind == 1 /* GG_E_VAR */ && !nullext && e->varattno >= 1 && e->varattno <= d->natts) ? d->attrs[e->varattno - 1].attnotnull : 0;
 	}
+	set_rows_layout(s, hj->numTargets, types, notnull);
 	return 0;
 }
 
@@ -542,75 +548,68 @@ static int has_numeric_agg(const gg_agg *agg)
 	return 0;
 }
 
-/* An Agg directly under a Sort or a Limit finalises its groups on the device into datum rows, which the node above sorts or
- * windows in place (only the Limit's window comes to the host).  Decided from the plan alone, so every segment decides alike:
- * a one-stage Agg over a scan or a join, or a FINAL Agg that combines device group records; no numeric aggregate (finalised on
- * the host only); and a device library with the entry points.  Otherwise the Agg hands up host rows, as it always did. */
-static void mark_agg_rows(GgPlanState *ch)
-{
-	int ok;
-	if (ch->having) return;                      /* decided at its own init: it always hands up (filtered) device rows */
-	if (!gg_scanagg_datumrows || !gg_joinagg_datumrows || !gg_groups_datumrows) return;
-	ok = ((ch->kind == K_SCANAGG || ch->kind == K_JOINAGG) && ch->agg.aggstage == GG_AGGSTAGE_NORMAL) ||
-	     (ch->kind == K_AGGFINAL && ch->dev_groups);
-	ch->agg_rows = ok && !has_numeric_agg(&ch->agg) && ch->agg.numCols + ch->agg.numAggs > 0;
-}
-
 /* The GG_FMT_DATUMROWS descriptor of an Agg's finalised rows: its output columns as set_layout_types types them.  NOT NULL
  * only where it is certain: count(*) and count(x) are never NULL; a key or any other aggregate may be (a NULL grouping value,
- * an aggregate over no non-NULL input).  A wrong NOT NULL would select a consumer's NULL-free kernel variant over NULLs. */
+ * an aggregate over no non-NULL input). */
 static int agg_rows_desc(GgPlanState *s)
 {
-	int c;
+	int8_t notnull[GG_MAX_OUTCOLS] = { 0 };
+	int i;
 	if (set_layout_types(s)) return -1;
 	if (s->ncols > GG_MAX_ATTS) { exec_fail(GG_ERR_UNSUPPORTED, "Agg with %d output columns (datum rows carry up to %d)", s->ncols, GG_MAX_ATTS); return -1; }
-	memset(&s->rows_desc, 0, sizeof s->rows_desc);
-	s->rows_desc.natts = s->ncols;
-	s->rows_desc.format = GG_FMT_DATUMROWS;
-	for (c = 0; c < s->ncols; c++)
-	{
-		gg_attr *a = &s->rows_desc.attrs[c];
-		const int i = c - s->agg.numCols;
-		a->atttypid = s->typid[c]; a->atttypmod = -1; a->attlen = 8; a->attalign = 'd'; a->attbyval = 1;
-		a->attnotnull = i >= 0 && (s->agg.aggs[i].aggfnoid == GG_AGG_COUNT_STAR || s->agg.aggs[i].aggfnoid == GG_AGG_COUNT_ANY);
-	}
-	s->rows_ncols = s->ncols;
+	for (i = 0; i < s->agg.numAggs; i++)
+		notnull[s->agg.numCols + i] = s->agg.aggs[i].aggfnoid == GG_AGG_COUNT_STAR || s->agg.aggs[i].aggfnoid == GG_AGG_COUNT_ANY;
+	set_rows_layout(s, s->ncols, s->typid, notnull);
 	return 0;
 }
 
-/* An Agg's HAVING (plan.qual; nodeAgg.c:1092 ExecQual over every finalised group).  Decided from the plan alone, so every
- * segment decides alike: the Agg always hands up its groups as device datum rows, filtered by the qual on the device
- * (gg_rowfilter); a FINAL Agg whose groups end up finalised on the host uploads them once and filters them the same way.  What
- * cannot take that path is refused: no path runs the Agg with its qual dropped. */
-static int init_having(GgPlanState *s, int32_t qual)
+/* What an Agg hands up, decided at the end of its init from the plan alone, so every segment decides alike.
+ * With a HAVING (plan.qual; nodeAgg.c:1092 ExecQual over every finalised group) it always hands up its groups as device datum
+ * rows, filtered by the qual on the device (gg_rowfilter); a FINAL Agg whose groups end up finalised on the host uploads them
+ * once and filters them the same way.  What cannot take that path is refused: no path runs the Agg with its qual dropped.
+ * Without one, when the node above reads device rows: a one-stage Agg over a scan or a join, or a FINAL Agg that combines
+ * device group records, finalises its groups on the device into datum rows, which the node above sorts, windows or joins in
+ * place; not with a numeric aggregate (finalised on the host only).  Otherwise the Agg hands up host rows. */
+static int init_agg_rows(GgPlanState *s, int32_t qual, int want)
 {
 	int rc;
-	if (s->agg.aggstage == GG_AGGSTAGE_PARTIAL)
-	{ exec_fail(GG_ERR_UNSUPPORTED, "a PARTIAL-stage Agg with a qual (HAVING belongs to the stage that finalises the groups)"); return -1; }
-	if (has_numeric_agg(&s->agg))
-	{ exec_fail(GG_ERR_UNSUPPORTED, "Agg with a qual: numeric aggregates have no device datum row to filter"); return -1; }
-	if (s->agg.numCols + s->agg.numAggs < 1) { exec_fail(GG_ERR_UNSUPPORTED, "Agg with a qual and no output columns"); return -1; }
-	if (!gg_rowfilter_create || !gg_rowfilter_run || !gg_rowfilter_free || !gg_relation_load || !gg_scanagg_datumrows || !gg_joinagg_datumrows ||
-	    !gg_groups_datumrows)
-	{ exec_fail(GG_ERR_UNSUPPORTED, "Agg with a qual: the device library has no row filter or no aggregate datum rows"); return -1; }
+	if (qual != -1)
+	{
+		if (s->agg.aggstage == GG_AGGSTAGE_PARTIAL)
+		{ exec_fail(GG_ERR_UNSUPPORTED, "a PARTIAL-stage Agg with a qual (HAVING belongs to the stage that finalises the groups)"); return -1; }
+		if (has_numeric_agg(&s->agg))
+		{ exec_fail(GG_ERR_UNSUPPORTED, "Agg with a qual: numeric aggregates have no device datum row to filter"); return -1; }
+		if (s->agg.numCols + s->agg.numAggs < 1) { exec_fail(GG_ERR_UNSUPPORTED, "Agg with a qual and no output columns"); return -1; }
+		if (!lib_has_rowfilter() || !lib_has_agg_rows())
+		{ exec_fail(GG_ERR_UNSUPPORTED, "Agg with a qual: the device library has no row filter or no aggregate datum rows"); return -1; }
+		s->agg_rows = WANT_ROWS_ONLY;
+	}
+	else if (want != WANT_HOST && lib_has_agg_rows() && !has_numeric_agg(&s->agg) && s->agg.numCols + s->agg.numAggs > 0 &&
+	         (((s->kind == K_SCANAGG || s->kind == K_JOINAGG) && s->agg.aggstage == GG_AGGSTAGE_NORMAL) || (s->kind == K_AGGFINAL && s->dev_groups)))
+		s->agg_rows = want;
+	if (want == WANT_ROWS_ONLY && !s->agg_rows)
+	{
+		exec_fail(GG_ERR_UNSUPPORTED, "HashJoin over an Agg: only a one-stage Agg over a scan or a join, or a FINAL Agg over device "
+		          "group records, without numeric aggregates, delivers its groups as device rows");
+		return -1;
+	}
+	if (!s->agg_rows) return 0;
 	if (agg_rows_desc(s)) return -1;
+	if (qual == -1) return 0;
 	rc = gg_rowfilter_create(s->estate->engine, &s->rows_desc, qual, s->estate->pool, &s->having);
 	if (rc != GG_OK) { s->having = NULL; exec_fail(rc, "Agg qual: %s", gg_last_error()); return -1; }
-	s->agg_rows = 1;
 	if (s->kind != K_AGGFINAL) s->dev_groups = 0;     /* a FINAL Agg keeps dev_groups: it says how it combines its input */
 	return 0;
 }
 
-/* The GG_FMT_DATUMROWS descriptor of the rows a node hands up, known at init: a row producer's own, an Agg's output columns,
- * and through a Sort, a Limit or a Motion that of the node below */
+/* The GG_FMT_DATUMROWS descriptor of the rows a node hands up, known at init: that of the producer below a Sort, a Limit or a
+ * Motion of host rows.  An Agg that hands up host rows has none yet: the WindowAgg above uploads them in this layout. */
 static int node_rows_desc(GgPlanState *s, gg_tupdesc *d)
 {
 	if (s->kind == K_SORT || s->kind == K_LIMIT || (s->kind == K_MOTION && !s->rows_scan)) return node_rows_desc(s->child, d);
 	if (s->kind == K_SCANAGG || s->kind == K_JOINAGG || s->kind == K_AGGFINAL)
 	{
-		/* the descriptor of its output columns (a HAVING's init made it already); an Agg that hands up host rows keeps no row width */
-		if (!s->having && agg_rows_desc(s)) return -1;
-		if (!s->agg_rows) s->rows_ncols = 0;
+		if (!s->agg_rows && agg_rows_desc(s)) return -1;
 	}
 	else if (s->kind != K_SCANROWS && s->kind != K_MOTION && s->kind != K_JOINROWS && s->kind != K_WINDOW)
 	{ exec_fail(GG_ERR_UNSUPPORTED, "WindowAgg: node kind %d below it delivers no rows", s->kind); return -1; }
@@ -642,11 +641,13 @@ static int init_window(GgPlanState *s, GgPlan *node, int eflags, int depth)
 	const gg_window *w = &wn->win;
 	GgEState *es = s->estate;
 	gg_tupdesc in;
+	int32_t types[GG_MAX_ATTS];
+	int8_t notnull[GG_MAX_ATTS] = { 0 };
 	int i, a, rc;
 	s->kind = K_WINDOW;
-	if (!gg_window_create || !gg_window_run || !gg_window_free || !gg_relation_load)
+	if (!lib_has_window())
 	{ exec_fail(GG_ERR_UNSUPPORTED, "WindowAgg: the device library has no window functions"); return -1; }
-	if (node->qual != -1 && (!gg_rowfilter_create || !gg_rowfilter_run || !gg_rowfilter_free))
+	if (node->qual != -1 && !lib_has_rowfilter())
 	{ exec_fail(GG_ERR_UNSUPPORTED, "WindowAgg with a qual: the device library has no row filter"); return -1; }
 	if (w->numFuncs < 1 || w->numFuncs > GG_MAX_WINFUNCS)
 	{ exec_fail(GG_ERR_UNSUPPORTED, "WindowAgg with %d window functions (1..%d)", w->numFuncs, GG_MAX_WINFUNCS); return -1; }
@@ -673,25 +674,16 @@ static int init_window(GgPlanState *s, GgPlan *node, int eflags, int depth)
 		exec_fail(GG_ERR_UNSUPPORTED, "WindowAgg: the node below must be a Sort on the partition columns, then the order columns");
 		return -1;
 	}
-	if (!(s->child = init_node(node->lefttree, es, eflags, depth + 1))) return -1;
-	mark_agg_rows(s->child);
+	if (!(s->child = init_node(node->lefttree, es, eflags, depth + 1, WANT_ROWS))) return -1;
 	if (node_rows_desc(s->child, &in)) return -1;
 	if (in.natts + w->numFuncs > GG_MAX_ATTS)
 	{ exec_fail(GG_ERR_UNSUPPORTED, "WindowAgg with %d output columns (datum rows carry up to %d)", in.natts + w->numFuncs, GG_MAX_ATTS); return -1; }
 	rc = gg_window_create(es->engine, &in, w, es->pool, &s->win);
 	if (rc != GG_OK) { s->win = NULL; exec_fail(rc, "WindowAgg: %s", gg_last_error()); return -1; }
-	s->rows_desc = in;
-	for (i = 0; i < in.natts; i++) s->typid[i] = in.attrs[i].atttypid;
-	for (i = 0; i < w->numFuncs; i++)
-	{
-		gg_attr *at = &s->rows_desc.attrs[in.natts + i];
-		memset(at, 0, sizeof *at);
-		at->atttypid = w->funcs[i].wintype; at->atttypmod = -1; at->attlen = 8; at->attalign = 'd'; at->attbyval = 1;
-		s->typid[in.natts + i] = w->funcs[i].wintype;
-	}
-	s->rows_desc.natts = in.natts + w->numFuncs;
-	s->ncols = s->rows_ncols = s->rows_desc.natts;
-	s->rows_nsegs = 1;
+	/* the child's columns as they are, then one column per function (never NOT NULL: lag / lead, an empty frame) */
+	for (i = 0; i < in.natts; i++) { types[i] = in.attrs[i].atttypid; notnull[i] = in.attrs[i].attnotnull; }
+	for (i = 0; i < w->numFuncs; i++) types[in.natts + i] = w->funcs[i].wintype;
+	set_rows_layout(s, in.natts + w->numFuncs, types, notnull);
 	if (node->qual != -1)
 	{
 		rc = gg_rowfilter_create(es->engine, &s->rows_desc, node->qual, es->pool, &s->having);
@@ -700,7 +692,7 @@ static int init_window(GgPlanState *s, GgPlan *node, int eflags, int depth)
 	return 0;
 }
 
-static GgPlanState *init_node(GgPlan *node, GgEState *estate, int eflags, int depth)
+static GgPlanState *init_node(GgPlan *node, GgEState *estate, int eflags, int depth, int want)
 {
 	GgPlanState *s;
 	if (!node) return NULL;                                   /* ExecInitNode(NULL) is NULL, execProcnode.c:268 */
@@ -736,7 +728,7 @@ static GgPlanState *init_node(GgPlan *node, GgEState *estate, int eflags, int de
 			{
 				/* the receiving half of a two-stage aggregate: combine what the Motion below delivers */
 				s->kind = K_AGGFINAL;
-				s->child = init_node(below, estate, eflags, depth + 1);
+				s->child = init_node(below, estate, eflags, depth + 1, WANT_HOST);
 				if (!s->child) goto fail;
 				{
 					/* device path: the child delivers group records of a PARTIAL stage with these very aggregates */
@@ -766,7 +758,7 @@ static GgPlanState *init_node(GgPlan *node, GgEState *estate, int eflags, int de
 			exec_fail(GG_ERR_UNSUPPORTED, "Agg: child node type %d is not on the accelerated path", below ? (int) below->type : 0);
 			goto fail;
 		agg_qual:
-			if (node->qual != -1 && init_having(s, node->qual)) goto fail;
+			if (init_agg_rows(s, node->qual, want)) goto fail;
 			return s;
 		}
 		case T_GgSort:
@@ -775,19 +767,17 @@ static GgPlanState *init_node(GgPlan *node, GgEState *estate, int eflags, int de
 			if (so->numCols < 1 || so->numCols > GG_MAX_SORTKEYS) { exec_fail(GG_ERR_UNSUPPORTED, "Sort with %d keys", so->numCols); goto fail; }
 			s->kind = K_SORT;
 			s->sort_bound = GG_NO_BOUND;
-			s->child = init_node(node->lefttree, estate, eflags, depth + 1);
+			s->child = init_node(node->lefttree, estate, eflags, depth + 1, WANT_ROWS);
 			if (!s->child) goto fail;
-			mark_agg_rows(s->child);
 			return s;
 		}
 		case T_GgLimit:
 			if (!node->lefttree) { exec_fail(GG_ERR_ARG, "Limit without a child"); goto fail; }
-			if (node->lefttree->type == T_GgSort && (!gg_sort_rows_bounded || !gg_sort_datumrows_bounded))
+			if (node->lefttree->type == T_GgSort && !lib_has_bounded_sort())
 			{ exec_fail(GG_ERR_UNSUPPORTED, "Limit over a Sort: the device library has no bounded sort"); goto fail; }
 			s->kind = K_LIMIT;
-			s->child = init_node(node->lefttree, estate, eflags, depth + 1);
+			s->child = init_node(node->lefttree, estate, eflags, depth + 1, WANT_ROWS);
 			if (!s->child) goto fail;
-			mark_agg_rows(s->child);
 			return s;
 		case T_GgMotion:
 		{
@@ -797,7 +787,7 @@ static GgPlanState *init_node(GgPlan *node, GgEState *estate, int eflags, int de
 			if (mo->motionType == GG_MOTIONTYPE_HASH && (mo->numHashCols < 1 || mo->numHashCols > GG_MAX_KEYS))
 			{ exec_fail(GG_ERR_UNSUPPORTED, "Redistribute Motion with %d hash columns", mo->numHashCols); goto fail; }
 			s->kind = K_MOTION;
-			s->child = init_node(node->lefttree, estate, eflags, depth + 1);
+			s->child = init_node(node->lefttree, estate, eflags, depth + 1, WANT_HOST);
 			if (!s->child) goto fail;
 			s->agg = s->child->agg;
 			{
@@ -1030,18 +1020,44 @@ static int run_child(GgPlanState *s)
 	return 0;
 }
 
+/* *buf, a buffer this node owns, made to hold nrows datum rows of W words and `slack` (> 0) bytes past them in whole 32 KB
+ * blocks: kept when it does already, created anew when it does not.  The blocks the rows and the slack take; 0: it failed. */
+static uint64_t reserve_rows(GgPlanState *s, gg_relation **buf, uint64_t nrows, uint64_t W, uint64_t slack, const char *what)
+{
+	const uint64_t nb = (nrows * W * 8 + slack + GG_BLCKSZ - 1) / GG_BLCKSZ;
+	int rc;
+	if (*buf && gg_relation_nblocks(*buf) >= nb) return nb;
+	if (*buf) gg_relation_free(*buf);
+	rc = gg_relation_create(s->estate->engine, nb, buf);
+	if (rc != GG_OK) { *buf = NULL; exec_fail(rc, "%s: %s", what, gg_last_error()); return 0; }
+	return nb;
+}
+
+/* n datum rows of s's layout at the start of `rows` handed up as s->rows_rel: through the node's qual first, when it has one (an
+ * Agg's HAVING, a WindowAgg's qual), so that only the rows it passes reach the node above */
+static int hand_up_rows(GgPlanState *s, gg_relation *rows, uint64_t n)
+{
+	int rc = GG_OK;
+	if (s->having) rc = gg_rowfilter_run(s->having, rows, n, &rows, &n);
+	if (rc == GG_OK) rc = gg_relation_attach_rows(s->estate->engine, gg_relation_device_ptr(rows), n, s->rows_desc.natts, &s->rows_rel);
+	if (rc != GG_OK) { s->rows_rel = NULL; exec_fail(rc, "%s", gg_last_error()); return -1; }
+	s->rows_n = n;
+	s->result = R_ROWS;
+	return 0;
+}
+
 /* ---- datum rows on the device: SeqScan projection, optionally partitioned for a Redistribute Motion ---- */
 static int run_rows_node(GgPlanState *s)
 {
 	GgEState *es = s->estate;
 	GgSeqScan *sc = s->rows_scan;
 	const int N = s->rows_nsegs;
-	const int W = 1 + s->rows_ncols;
+	const int W = 1 + s->rows_desc.natts;
 	const uint64_t nblocks = gg_relation_nblocks(s->rel);
 	gg_scan scan;
 	int32_t hashkeys[GG_MAX_KEYS];
 	int nkeys = 0, c, rc, attempt;
-	uint64_t counts[1024], offs[1024];
+	uint64_t counts[1024], offs[1024], recv_rows;
 	if (N > 1024) { exec_fail(GG_ERR_UNSUPPORTED, "more than 1024 segments"); return -1; }
 	memset(&scan, 0, sizeof scan);
 	scan.desc = sc->desc; scan.qual = sc->plan.qual;
@@ -1053,106 +1069,96 @@ static int run_rows_node(GgPlanState *s)
 	else
 		hashkeys[nkeys++] = s->rows_targets[0];          /* one destination: the key only feeds jump_consistent_hash(h, 1) = 0 */
 	drop_device_results(s);
+	if (!s->rows_cap)
+	{
+		/* the line pointers bound the rows; a hash spreads them evenly over the destinations (10 % + 8192 slack each) */
+		uint64_t nlp = 0;
+		rc = gg_relation_count_rows(s->rel, &nlp);
+		if (rc != GG_OK) { exec_fail(rc, "%s", gg_last_error()); return -1; }
+		/* + 1/4: a hash does not spread perfectly, and the sending kernel leaves up to 1/8 of a region as dead slots */
+		s->rows_cap = (nlp / (uint64_t) N + nlp / (uint64_t) (4 * N) + 8192) * (uint64_t) N;
+	}
 	for (attempt = 0; ; attempt++)
 	{
-		if (!s->rows_send)
-		{
-			uint64_t words;
-			if (!s->rows_cap)
-			{
-				/* the line pointers bound the rows; a hash spreads them evenly over the destinations (10 % + 8192 slack each) */
-				uint64_t nlp = 0;
-				rc = gg_relation_count_rows(s->rel, &nlp);
-				if (rc != GG_OK) { exec_fail(rc, "%s", gg_last_error()); return -1; }
-				/* + 1/4: a hash does not spread perfectly, and the sending kernel leaves up to 1/8 of a region as dead slots */
-				s->rows_cap = (nlp / (uint64_t) N + nlp / (uint64_t) (4 * N) + 8192) * (uint64_t) N;
-			}
-			words = s->rows_cap * (uint64_t) W + 8;
-			rc = gg_relation_create(es->engine, (words * 8 + GG_BLCKSZ - 1) / GG_BLCKSZ, &s->rows_send);
-			if (rc != GG_OK) { exec_fail(rc, "Motion send buffer: %s", gg_last_error()); return -1; }
-		}
-		rc = gg_motion_partition(es->engine, &scan, es->pool, hashkeys, nkeys, s->rows_targets, s->rows_ncols, N, s->rel, 0, nblocks,
+		if (!reserve_rows(s, &s->rows_send, s->rows_cap, W, 64, "Motion send buffer")) return -1;
+		rc = gg_motion_partition(es->engine, &scan, es->pool, hashkeys, nkeys, s->rows_targets, s->rows_desc.natts, N, s->rel, 0, nblocks,
 		                         gg_relation_device_ptr(s->rows_send), s->rows_cap, counts, offs);
 		if (rc != GG_ERR_NOMEM || attempt >= 2) break;
-		gg_relation_free(s->rows_send); s->rows_send = NULL;
 		s->rows_cap *= 2;
 	}
 	if (rc != GG_OK) { exec_fail(rc, "%s", gg_last_error()); return -1; }
-	if (N == 1)
-	{
-		s->rows_n = counts[0];
-		rc = gg_relation_attach_rows(es->engine, gg_relation_device_ptr(s->rows_send), s->rows_n, s->rows_ncols, &s->rows_rel);
-		if (rc != GG_OK) { exec_fail(rc, "%s", gg_last_error()); return -1; }
-		return 0;
-	}
-	for (attempt = 0; ; attempt++)
+	if (N == 1) return hand_up_rows(s, s->rows_send, counts[0]);
+	for (attempt = 0, recv_rows = s->rows_cap; ; attempt++)
 	{
 		const uint64_t region_cap = (s->rows_cap / (uint64_t) N) & ~1ull;
-		uint64_t recv_cap;
-		if (!s->rows_recv)
-		{
-			rc = gg_relation_create(es->engine, ((s->rows_cap * (uint64_t) W + 8) * 8 + GG_BLCKSZ - 1) / GG_BLCKSZ, &s->rows_recv);
-			if (rc != GG_OK) { exec_fail(rc, "Motion receive buffer: %s", gg_last_error()); return -1; }
-		}
+		uint64_t recv_cap, n = 0;
+		if (!reserve_rows(s, &s->rows_recv, recv_rows, W, 64, "Motion receive buffer")) return -1;
 		recv_cap = gg_relation_nblocks(s->rows_recv) * (uint64_t) GG_BLCKSZ / 8 / (uint64_t) W - 2;
 		rc = gg_ic_exchange_rows(es->interconnect, gg_relation_device_ptr(s->rows_send), counts, region_cap, W,
-		                         gg_relation_device_ptr(s->rows_recv), recv_cap, &s->rows_n);
+		                         gg_relation_device_ptr(s->rows_recv), recv_cap, &n);
+		if (rc == GG_OK) return hand_up_rows(s, s->rows_recv, n);
 		if (rc != GG_ERR_NOMEM || attempt >= 1) break;
 		/* every segment saw the overflow: all of them come back with a receive buffer twice the size */
-		{
-			const uint64_t nb = gg_relation_nblocks(s->rows_recv) * 2;
-			gg_relation_free(s->rows_recv); s->rows_recv = NULL;
-			rc = gg_relation_create(es->engine, nb, &s->rows_recv);
-			if (rc != GG_OK) { exec_fail(rc, "Motion receive buffer: %s", gg_last_error()); return -1; }
-		}
+		recv_rows = 2 * gg_relation_nblocks(s->rows_recv) * (uint64_t) GG_BLCKSZ / 8 / (uint64_t) W;
 	}
-	if (rc != GG_OK) { exec_fail(rc, "%s", gg_last_error()); return -1; }
-	rc = gg_relation_attach_rows(es->engine, gg_relation_device_ptr(s->rows_recv), s->rows_n, s->rows_ncols, &s->rows_rel);
-	if (rc != GG_OK) { exec_fail(rc, "%s", gg_last_error()); return -1; }
-	return 0;
+	exec_fail(rc, "%s", gg_last_error());
+	return -1;
 }
 
-/* the device buffer that holds a rows node's datum rows */
-static gg_relation *rows_buffer(const GgPlanState *s)
+/* s's result = live datum rows [skip, skip + take) of ch (s itself, or the node below), copied from the device a few 32 KB blocks
+ * at a time: only the leading blocks that hold them, never the whole buffer.  *pulled: live rows of ch read (skip + the rows
+ * taken). */
+static int rows_window_to_host(GgPlanState *s, const GgPlanState *ch, uint64_t skip, uint64_t take, uint64_t *pulled)
 {
-	if (s->kind == K_JOINROWS || s->kind == K_WINDOW || s->agg_rows) return s->rows_rel;   /* the join's / window's / Agg's own output */
-	return s->rows_recv && s->rows_nsegs > 1 ? s->rows_recv : s->rows_send;
+	const int32_t ncols = ch->rows_desc.natts;
+	const uint64_t W = 1 + (uint64_t) ncols, nrows = ch->rows_n;
+	const uint64_t total_nb = (nrows * W * 8 + GG_BLCKSZ - 1) / GG_BLCKSZ;
+	const uint64_t need = skip + take < skip ? UINT64_MAX : skip + take;
+	const uint64_t cap = take < nrows ? take : nrows;
+	gg_relation *src = ch->rows_rel;
+	uint64_t *buf = NULL, have_nb = 0, r = 0, live = 0, out = 0;
+	int c, rc;
+	if (alloc_result(s, (int64_t) cap, ncols)) { exec_fail(GG_ERR_NOMEM, "out of memory"); return -1; }
+	while (r < nrows && live < need)
+	{
+		/* every block so far held rows; ask for enough new blocks to hold the rows still wanted if none of them were dead */
+		const uint64_t rows_wanted = need - live < nrows - r ? need - live : nrows - r;
+		uint64_t want_nb = ((r + rows_wanted) * W * 8 + GG_BLCKSZ - 1) / GG_BLCKSZ;
+		uint64_t *nbuf;
+		if (want_nb <= have_nb) want_nb = have_nb + 1;
+		if (want_nb > total_nb) want_nb = total_nb;
+		nbuf = realloc(buf, (size_t) want_nb * GG_BLCKSZ);
+		if (!nbuf) { free(buf); exec_fail(GG_ERR_NOMEM, "out of memory"); return -1; }
+		buf = nbuf;
+		rc = gg_relation_read(src, have_nb, (uint8_t *) buf + have_nb * GG_BLCKSZ, want_nb - have_nb);
+		if (rc != GG_OK) { free(buf); exec_fail(rc, "%s", gg_last_error()); return -1; }
+		have_nb = want_nb;
+		for (; r < nrows && (r + 1) * W * 8 <= have_nb * GG_BLCKSZ && live < need; r++)
+		{
+			if (buf[r * W] & GG_DATUMROW_DEAD) continue;            /* a slot the sending kernel claimed and did not fill */
+			if (live++ < skip) continue;
+			for (c = 0; c < ncols; c++)
+			{
+				const uint64_t v = buf[r * W + 1 + c];
+				s->values[out * ncols + c] = (int64_t) v;
+				s->isnull[out * ncols + c] = (uint8_t) ((buf[r * W] >> c) & 1);
+				if (is_string_type(ch->typid[c])) s->lens[out * ncols + c] = packed_len(v);
+			}
+			out++;
+		}
+	}
+	free(buf);
+	s->nrows = (int64_t) out;
+	s->result = R_HOST;
+	*pulled = live;
+	return 0;
 }
 
 /* device rows -> host result arrays (only when a rows node sits at the top of what the caller drives) */
 static int rows_to_host(GgPlanState *s)
 {
-	const int W = 1 + s->rows_ncols;
-	const uint64_t n = s->rows_n;
-	const uint64_t bytes = n * (uint64_t) W * 8;
-	const uint64_t nb = (bytes + GG_BLCKSZ - 1) / GG_BLCKSZ;
-	uint64_t *buf, r;
-	int c, rc;
-	if (alloc_result(s, (int64_t) n, s->rows_ncols)) { exec_fail(GG_ERR_NOMEM, "out of memory"); return -1; }
-	if (n)
-	{
-		uint64_t live = 0;
-		buf = malloc((size_t) nb * GG_BLCKSZ);
-		if (!buf) { exec_fail(GG_ERR_NOMEM, "out of memory"); return -1; }
-		rc = gg_relation_read(rows_buffer(s), 0, buf, nb);
-		if (rc != GG_OK) { free(buf); exec_fail(rc, "%s", gg_last_error()); return -1; }
-		for (r = 0; r < n; r++)
-		{
-			if (buf[r * W] & GG_DATUMROW_DEAD) continue;          /* a slot the sending kernel claimed and did not fill */
-			for (c = 0; c < s->rows_ncols; c++)
-			{
-				const uint64_t v = buf[r * W + 1 + c];
-				s->values[live * s->rows_ncols + c] = (int64_t) v;
-				s->isnull[live * s->rows_ncols + c] = (uint8_t) ((buf[r * W] >> c) & 1);
-				if (is_string_type(s->typid[c])) s->lens[live * s->rows_ncols + c] = packed_len(v);
-			}
-			live++;
-		}
-		s->nrows = (int64_t) live;
-		free(buf);
-	}
-	s->rows_ready = 1;
-	return 0;
+	uint64_t pulled;
+	return rows_window_to_host(s, s, 0, UINT64_MAX, &pulled);
 }
 
 /* a failure reading a node's aggregate rows: this segment's own earlier failure, when there was one, is the better message */
@@ -1162,45 +1168,29 @@ static void groups_fail(const GgPlanState *s, int rc)
 	else exec_fail(rc, "%s", gg_last_error());
 }
 
-/* an Agg's s->rows_n finalised rows (a datum-row view) handed up as s->rows_rel: through its HAVING filter first, when it has one,
- * so that only the groups whose qual is TRUE reach the node above */
-static int hand_up_rows(GgPlanState *s, gg_relation *rows)
-{
-	int rc = GG_OK;
-	s->rows_ncols = s->ncols;
-	s->rows_nsegs = 1;
-	if (s->having) rc = gg_rowfilter_run(s->having, rows, s->rows_n, &rows, &s->rows_n);
-	if (rc == GG_OK) rc = gg_relation_attach_rows(s->estate->engine, gg_relation_device_ptr(rows), s->rows_n, s->rows_ncols, &s->rows_rel);
-	if (rc != GG_OK) { s->rows_rel = NULL; exec_fail(rc, "%s", gg_last_error()); return -1; }
-	s->rows_ready = 0;
-	return 0;
-}
-
 /* the Agg's groups as device datum rows (agg_rows): the view its pipeline or group set hands out, wrapped for the node above */
 static int agg_datumrows(GgPlanState *s)
 {
 	gg_relation *out = NULL;
+	uint64_t n = 0;
 	int rc;
 	if (set_layout_types(s)) return -1;
-	if (s->groups) rc = gg_groups_datumrows(s->groups, &out, &s->rows_n);
-	else if (s->kind == K_SCANAGG) rc = gg_scanagg_datumrows(s->sa, &out, &s->rows_n);
-	else rc = gg_joinagg_datumrows(s->ja, &out, &s->rows_n);
+	if (s->groups) rc = gg_groups_datumrows(s->groups, &out, &n);
+	else if (s->kind == K_SCANAGG) rc = gg_scanagg_datumrows(s->sa, &out, &n);
+	else rc = gg_joinagg_datumrows(s->ja, &out, &n);
 	if (rc != GG_OK) { groups_fail(s, rc); return -1; }
-	return hand_up_rows(s, out);
+	return hand_up_rows(s, out, n);
 }
 
-/* the host rows of src uploaded once as datum rows into s->rows_send; *view wraps them (the caller frees it) */
+/* the host rows of src (s itself, or the node below) uploaded once as datum rows into s->rows_send; *view wraps them (the caller
+ * frees it): the rows a FINAL Agg hands up, or those a WindowAgg windows */
 static int upload_host_rows(GgPlanState *s, const GgPlanState *src, gg_relation **view)
 {
-	GgEState *es = s->estate;
 	const uint64_t n = src->nrows > 0 ? (uint64_t) src->nrows : 0, W = 1 + (uint64_t) src->ncols;
-	const uint64_t nb = (n * W * 8 + 16 + GG_BLCKSZ - 1) / GG_BLCKSZ;
-	uint64_t *buf, r;
+	uint64_t *buf, r, nb;
 	int c, rc;
 	*view = NULL;
-	if (s->rows_send && gg_relation_nblocks(s->rows_send) < nb) { gg_relation_free(s->rows_send); s->rows_send = NULL; }
-	if (!s->rows_send && (rc = gg_relation_create(es->engine, nb, &s->rows_send)) != GG_OK)
-	{ s->rows_send = NULL; exec_fail(rc, "rows: %s", gg_last_error()); return -1; }
+	if (!(nb = reserve_rows(s, &s->rows_send, n, W, 16, "rows"))) return -1;
 	buf = calloc((size_t) nb, GG_BLCKSZ);
 	if (!buf) { exec_fail(GG_ERR_NOMEM, "out of memory"); return -1; }
 	for (r = 0; r < n; r++)
@@ -1211,21 +1201,20 @@ static int upload_host_rows(GgPlanState *s, const GgPlanState *src, gg_relation 
 		}
 	rc = gg_relation_load(s->rows_send, 0, buf, nb);              /* pageable: staged before the call returns, so buf can go */
 	free(buf);
-	if (rc == GG_OK) rc = gg_relation_attach_rows(es->engine, gg_relation_device_ptr(s->rows_send), n, src->ncols, view);
+	if (rc == GG_OK) rc = gg_relation_attach_rows(s->estate->engine, gg_relation_device_ptr(s->rows_send), n, src->ncols, view);
 	if (rc != GG_OK) { *view = NULL; exec_fail(rc, "rows: %s", gg_last_error()); return -1; }
 	return 0;
 }
 
 /* A FINAL Agg whose groups were finalised on the host (its child delivered host rows, or the slice was re-run with host-row
- * Motions), under a HAVING filter or a HashJoin: its host rows uploaded once as datum rows (into rows_send) and handed up as the
- * device path hands them up, so the qual is evaluated one way only */
+ * Motions), under a HAVING filter or a HashJoin: its host rows uploaded once and handed up as the device path hands them up, so
+ * the qual is evaluated one way only */
 static int upload_agg_rows(GgPlanState *s)
 {
 	gg_relation *view = NULL;
 	int rc;
 	if (upload_host_rows(s, s, &view)) return -1;
-	s->rows_n = s->nrows > 0 ? (uint64_t) s->nrows : 0;
-	rc = hand_up_rows(s, view);
+	rc = hand_up_rows(s, view, s->nrows > 0 ? (uint64_t) s->nrows : 0);
 	gg_relation_free(view);
 	return rc;
 }
@@ -1242,22 +1231,18 @@ static int run_window(GgPlanState *s)
 	drop_device_results(s);
 	if (run_child(s)) return -1;
 	s->nonreceiver = ch->nonreceiver;
-	if (ch->rows_rel && !ch->rows_ready) { in = ch->rows_rel; nin = ch->rows_n; }
+	if (ch->result == R_ROWS) { in = ch->rows_rel; nin = ch->rows_n; }
 	else
 	{
 		if (ensure_rows(ch) || upload_host_rows(s, ch, &up)) return -1;
 		in = up; nin = ch->nrows > 0 ? (uint64_t) ch->nrows : 0;
 	}
 	rc = gg_window_run(s->win, in, nin, &out, &nout);
-	s->win_ms = 0.0f;
-	if (rc == GG_OK && gg_engine_last_kernel_ms) (void) gg_engine_last_kernel_ms(es->engine, &s->win_ms);
-	if (rc == GG_OK && s->having) rc = gg_rowfilter_run(s->having, out, nout, &out, &nout);
-	if (rc == GG_OK) rc = gg_relation_attach_rows(es->engine, gg_relation_device_ptr(out), nout, s->rows_ncols, &s->rows_rel);
 	if (up) gg_relation_free(up);
-	if (rc != GG_OK) { s->rows_rel = NULL; exec_fail(rc, "%s", gg_last_error()); return -1; }
-	s->rows_n = nout;
-	s->rows_ready = 0;
-	return 0;
+	s->win_ms = 0.0f;
+	if (rc != GG_OK) { exec_fail(rc, "%s", gg_last_error()); return -1; }
+	if (gg_engine_last_kernel_ms) (void) gg_engine_last_kernel_ms(es->engine, &s->win_ms);
+	return hand_up_rows(s, out, nout);
 }
 
 /* a node's aggregate rows -> host result arrays, from its device group records (the one synchronisation of a
@@ -1297,9 +1282,9 @@ static int pipeline_groups(GgPlanState *s)
 
 static int ensure_rows(GgPlanState *s)
 {
-	if (s->rows_ready) return 0;
-	if (s->rows_rel || s->kind == K_SCANROWS || (s->kind == K_MOTION && s->rows_scan)) return rows_to_host(s);
-	if (s->groups) return aggrows_to_host(s);
+	if (s->result == R_HOST) return 0;
+	if (s->result == R_ROWS) return rows_to_host(s);
+	if (s->result == R_GROUPS) return aggrows_to_host(s);
 	exec_fail(GG_ERR_ARG, "node has no result");
 	return -1;
 }
@@ -1403,7 +1388,7 @@ static int motion_host_path(GgPlanState *s, int child_failed)
 		if (mo->numSortCols > GG_MAX_SORTKEYS) { exec_fail(GG_ERR_UNSUPPORTED, "Motion with %d merge keys", mo->numSortCols); return -1; }
 		if (sort_keys(keys, mo->sortKeys, mo->numSortCols, s, "Motion merge") || sort_host_rows(s, s, keys, mo->numSortCols, 0, GG_NO_BOUND)) return -1;
 	}
-	s->rows_ready = 1;
+	s->result = R_HOST;
 	return 0;
 }
 
@@ -1447,10 +1432,10 @@ static int run_agg_pipeline(GgPlanState *s)
 	{
 		/* the joined rows stay on the device for the node above (or come to the host once, at the top) */
 		gg_relation *out;
-		uint64_t live;
-		rc = gg_joinagg_rows(s->ja, &out, &s->rows_n, &live);
-		if (rc == GG_OK) rc = gg_relation_attach_rows(es->engine, gg_relation_device_ptr(out), s->rows_n, s->rows_ncols, &s->rows_rel);
-		if (rc != GG_OK) { s->rows_rel = NULL; exec_fail(rc, "%s", gg_last_error()); return -1; }
+		uint64_t n, live;
+		rc = gg_joinagg_rows(s->ja, &out, &n, &live);
+		if (rc != GG_OK) { exec_fail(rc, "%s", gg_last_error()); return -1; }
+		if (hand_up_rows(s, out, n)) return -1;
 		/* whether a segment batched depends on its own inner rows; a Motion below the Hash is a plan property, the same on
 		 * every segment, so a rescan re-runs that exchange everywhere or nowhere */
 		s->table_kept = gg_joinagg_nbatch(s->ja) == 1 && !has_motion(s->inner);
@@ -1464,7 +1449,7 @@ static int run_agg_pipeline(GgPlanState *s)
 		/* the records go straight into the Motion above; a pipeline that would have to be replayed says so in its
 		 * status, which makes that Motion (on every segment) fall back to host rows — where the fetch below runs */
 		if (set_layout_types(s)) return -1;
-		s->rows_ready = 0;
+		s->result = R_GROUPS;
 		return 0;
 	}
 	/* fetch decides whether the pipeline has to be replayed on a wider kernel variant (more groups than expected, a
@@ -1491,7 +1476,7 @@ static int run_final_agg(GgPlanState *s)
 		if (rc != GG_OK) { exec_fail(rc, "%s", gg_last_error()); return -1; }
 		if (s->agg_rows) return agg_datumrows(s);
 		if (set_layout_types(s)) return -1;
-		s->rows_ready = 0;
+		s->result = R_GROUPS;
 		return 0;
 	}
 	if (ensure_rows(ch)) return -1;
@@ -1500,8 +1485,8 @@ static int run_final_agg(GgPlanState *s)
 		/* the slice above a Gather exists only on the receiving segment (the QD in the reference): no rows here, not
 		 * even the empty-input row of a plain aggregate */
 		if (alloc_result(s, 0, ch->ncols)) { exec_fail(GG_ERR_NOMEM, "out of memory"); return -1; }
-		s->rows_ready = 1;
-		if (s->having || s->rows_required) { if (set_layout_types(s)) return -1; s->nrows = 0; return upload_agg_rows(s); }
+		s->result = R_HOST;
+		if (s->agg_rows == WANT_ROWS_ONLY) { if (set_layout_types(s)) return -1; s->nrows = 0; return upload_agg_rows(s); }
 		return 0;
 	}
 	part.aggstage = GG_AGGSTAGE_PARTIAL;      /* layout of the incoming rows */
@@ -1517,7 +1502,7 @@ static int run_final_agg(GgPlanState *s)
 	if (rc != GG_OK) { exec_fail(rc, "%s", gg_last_error()); free(out); return -1; }
 	rc = rows_from_aggrows(s, out, n);
 	free(out);
-	if (rc == 0 && (s->having || s->rows_required)) rc = upload_agg_rows(s);
+	if (rc == 0 && s->agg_rows == WANT_ROWS_ONLY) rc = upload_agg_rows(s);
 	return rc;
 }
 
@@ -1532,35 +1517,27 @@ static int run_sort(GgPlanState *s)
 	if (run_child(s)) return -1;
 	s->nonreceiver = ch->nonreceiver;
 	if (sort_keys(keys, so->keys, so->numCols, ch, "Sort")) return -1;
-	if (ch->rows_rel && !ch->rows_ready)
+	if (ch->result == R_ROWS)
 	{
 		/* the input is datum rows on the device (a row-producing SeqScan, or the Motion over one): sort them where they
 		 * are; the sorted rows stay on the device for the node above, or come to the host once, at the top */
-		const uint64_t W = 1 + (uint64_t) ch->rows_ncols;
+		const int32_t ncols = ch->rows_desc.natts;
 		const uint64_t nout = ch->rows_n < s->sort_bound ? ch->rows_n : s->sort_bound;
-		const uint64_t nb = (nout * W * 8 + 64 + GG_BLCKSZ - 1) / GG_BLCKSZ;
 		uint64_t live = 0;
 		drop_device_results(s);
-		if (s->rows_send && gg_relation_nblocks(s->rows_send) < nb) { gg_relation_free(s->rows_send); s->rows_send = NULL; }
-		if (!s->rows_send)
-		{
-			rc = gg_relation_create(es->engine, nb, &s->rows_send);
-			if (rc != GG_OK) { exec_fail(rc, "Sort result: %s", gg_last_error()); return -1; }
-		}
+		if (!reserve_rows(s, &s->rows_send, nout, 1 + (uint64_t) ncols, 64, "Sort result")) return -1;
 		/* bounded (a Limit above): only the first sort_bound rows of the order are selected, sorted and written */
 		if (s->sort_bound != GG_NO_BOUND)
-			rc = gg_sort_datumrows_bounded(es->engine, keys, so->numCols, ch->rows_ncols, gg_relation_device_ptr(ch->rows_rel), ch->rows_n,
+			rc = gg_sort_datumrows_bounded(es->engine, keys, so->numCols, ncols, gg_relation_device_ptr(ch->rows_rel), ch->rows_n,
 			                               s->sort_bound, gg_relation_device_ptr(s->rows_send), &live, NULL);
 		else
-			rc = gg_sort_datumrows(es->engine, keys, so->numCols, ch->rows_ncols, gg_relation_device_ptr(ch->rows_rel), ch->rows_n,
+			rc = gg_sort_datumrows(es->engine, keys, so->numCols, ncols, gg_relation_device_ptr(ch->rows_rel), ch->rows_n,
 			                       gg_relation_device_ptr(s->rows_send), &live, NULL);
 		if (rc != GG_OK) { exec_fail(rc, "%s", gg_last_error()); return -1; }
-		s->rows_n = live; s->rows_ncols = ch->rows_ncols; s->rows_nsegs = 1;
+		s->rows_desc = ch->rows_desc;
 		s->ncols = ch->ncols;
 		memcpy(s->typid, ch->typid, sizeof s->typid);
-		rc = gg_relation_attach_rows(es->engine, gg_relation_device_ptr(s->rows_send), live, ch->rows_ncols, &s->rows_rel);
-		if (rc != GG_OK) { exec_fail(rc, "%s", gg_last_error()); return -1; }
-		return 0;
+		return hand_up_rows(s, s->rows_send, live);
 	}
 	if (ensure_rows(ch)) return -1;
 	memcpy(s->typid, ch->typid, sizeof s->typid);
@@ -1573,57 +1550,11 @@ static int run_sort(GgPlanState *s)
 	/* bounded: when the bound's rows fit the operator's memory, one bounded sort and no runs at all (tuplesort_mk's bounded
 	 * heap never spills); otherwise each run keeps its first `bound` rows and the merge stops there */
 	if (sort_host_rows(s, ch, keys, so->numCols, run_rows, s->sort_bound)) return -1;
-	s->rows_ready = 1;
+	s->result = R_HOST;
 	return 0;
 }
 
 /* ---- Limit (nodeLimit.c): forward-only; the window [offset, offset + count) of the child's rows as host rows ---- */
-
-/* s's result = live datum rows [skip, skip + take) of ch, copied from the device a few 32 KB blocks at a time: only the leading
- * blocks that hold them, never the whole buffer.  *pulled: live rows of ch read (skip + the rows taken). */
-static int rows_window_to_host(GgPlanState *s, const GgPlanState *ch, uint64_t skip, uint64_t take, uint64_t *pulled)
-{
-	const uint64_t W = 1 + (uint64_t) ch->rows_ncols;
-	const uint64_t total_nb = (ch->rows_n * W * 8 + GG_BLCKSZ - 1) / GG_BLCKSZ;
-	const uint64_t need = skip + take < skip ? UINT64_MAX : skip + take;
-	gg_relation *src = rows_buffer(ch);
-	uint64_t *buf = NULL, have_nb = 0, r = 0, live = 0, out = 0;
-	int c, rc;
-	const uint64_t cap = take < (uint64_t) ch->rows_n ? take : (uint64_t) ch->rows_n;
-	if (alloc_result(s, (int64_t) cap, ch->rows_ncols)) { exec_fail(GG_ERR_NOMEM, "out of memory"); return -1; }
-	while (r < ch->rows_n && live < need)
-	{
-		/* every block so far held rows; ask for enough new blocks to hold the rows still wanted if none of them were dead */
-		const uint64_t rows_wanted = need - live < ch->rows_n - r ? need - live : ch->rows_n - r;
-		uint64_t want_nb = ((r + rows_wanted) * W * 8 + GG_BLCKSZ - 1) / GG_BLCKSZ;
-		uint64_t *nbuf;
-		if (want_nb <= have_nb) want_nb = have_nb + 1;
-		if (want_nb > total_nb) want_nb = total_nb;
-		nbuf = realloc(buf, (size_t) want_nb * GG_BLCKSZ);
-		if (!nbuf) { free(buf); exec_fail(GG_ERR_NOMEM, "out of memory"); return -1; }
-		buf = nbuf;
-		rc = gg_relation_read(src, have_nb, (uint8_t *) buf + have_nb * GG_BLCKSZ, want_nb - have_nb);
-		if (rc != GG_OK) { free(buf); exec_fail(rc, "%s", gg_last_error()); return -1; }
-		have_nb = want_nb;
-		for (; r < ch->rows_n && (r + 1) * W * 8 <= have_nb * GG_BLCKSZ && live < need; r++)
-		{
-			if (buf[r * W] & GG_DATUMROW_DEAD) continue;            /* a slot the sending kernel claimed and did not fill */
-			if (live++ < skip) continue;
-			for (c = 0; c < ch->rows_ncols; c++)
-			{
-				const uint64_t v = buf[r * W + 1 + c];
-				s->values[out * ch->rows_ncols + c] = (int64_t) v;
-				s->isnull[out * ch->rows_ncols + c] = (uint8_t) ((buf[r * W] >> c) & 1);
-				if (is_string_type(ch->typid[c])) s->lens[out * ch->rows_ncols + c] = packed_len(v);
-			}
-			out++;
-		}
-	}
-	free(buf);
-	s->nrows = (int64_t) out;
-	*pulled = live;
-	return 0;
-}
 
 static int run_limit(GgPlanState *s)
 {
@@ -1649,7 +1580,7 @@ static int run_limit(GgPlanState *s)
 		inherit_layout(s, ch);
 		if (alloc_result(s, 0, s->ncols > 0 ? s->ncols : 1)) { exec_fail(GG_ERR_NOMEM, "out of memory"); return -1; }
 		s->nonreceiver = ch->nonreceiver;
-		s->rows_ready = 1;
+		s->result = R_HOST;
 		return 0;
 	}
 	if (run_child(s)) return -1;
@@ -1657,7 +1588,7 @@ static int run_limit(GgPlanState *s)
 	inherit_layout(s, ch);
 	skip = (uint64_t) offset;
 	take = lp->hasCount ? (uint64_t) count : UINT64_MAX;
-	if (ch->rows_rel && !ch->rows_ready)
+	if (ch->result == R_ROWS)
 	{
 		if (rows_window_to_host(s, ch, skip, take, &pulled)) return -1;
 	}
@@ -1678,7 +1609,7 @@ static int run_limit(GgPlanState *s)
 	ch->instr_ntuples += (double) pulled;
 	/* the window is complete: the node below will not be read again (ExecLimit, nodeLimit.c:239-247) */
 	GgExecSquelchNode(ch);
-	s->rows_ready = 1;
+	s->result = R_HOST;
 	return 0;
 }
 
@@ -1714,7 +1645,7 @@ static int run_motion(GgPlanState *s)
 	if (s->nonreceiver) gg_groups_set_nonreceiver(s->groups);
 	/* a failed child left no layout: the rows this node would have handed up take it from the plan */
 	if (child_failed && set_layout_types(s)) return -1;
-	s->rows_ready = 0;
+	s->result = R_GROUPS;
 	return 0;
 }
 
@@ -1988,7 +1919,7 @@ int GgExecRecvTupleChunks(GgPlanState *s, const uint8_t *chunks, uint64_t nbytes
 	free(b);
 	if (rc != GG_OK) return (exec_fail(rc, "reading tuple chunks failed (%d)", rc), rc);
 	drop_device_results(s);
-	s->rows_ready = 1; s->done = 1; s->next = 0;
+	s->result = R_HOST; s->done = 1; s->next = 0;
 	return GG_OK;
 }
 
@@ -2009,7 +1940,7 @@ GgTupleTableSlot *GgExecProcNode(GgPlanState *s)
 			if (c != GG_OK) { exec_fail(c, "%s", gg_last_error()); return NULL; }
 			failed = run_node(s);                     /* the C wrapper on the Postgres side turns a failure into ereport(ERROR) */
 		}
-		if (!failed && !s->rows_ready)
+		if (!failed && s->result != R_HOST)
 		{
 			g_err[0] = 0; g_errcode = GG_OK;
 			failed = ensure_rows(s);
@@ -2063,7 +1994,7 @@ int GgExecReScan(GgPlanState *s)
 	drop_device_results(s);
 	if (s->sa) rc = gg_scanagg_reset(s->sa);
 	if (s->ja && rc == GG_OK) rc = gg_joinagg_reset(s->ja);
-	s->done = 0; s->squelched = 0; s->next = 0; s->nrows = 0; s->rows_ready = 0; s->markpos = 0;
+	s->done = 0; s->squelched = 0; s->next = 0; s->nrows = 0; s->markpos = 0;
 	return rc;
 }
 

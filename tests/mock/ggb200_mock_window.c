@@ -30,7 +30,7 @@ int gg_relation_create(gg_engine *e, uint64_t nblocks, gg_relation **out)
 
 int gg_relation_load(gg_relation *r, uint64_t first_block, const void *host_pages, uint64_t nblocks)
 {
-	if (!r->owned || first_block + nblocks > r->nblocks) { gg_set_error("mock: load outside the relation"); return GG_ERR_ARG; }
+	if (!r->owned || nblocks > r->nblocks || first_block > r->nblocks - nblocks) { gg_set_error("mock: load outside the relation"); return GG_ERR_ARG; }
 	memcpy(r->owned + first_block * GG_BLCKSZ, host_pages, (size_t) nblocks * GG_BLCKSZ);
 	return GG_OK;
 }
@@ -41,13 +41,18 @@ int gg_relation_attach_rows(gg_engine *e, void *rows, uint64_t nrows, int ncols,
 	(void) e;
 	if (!r) { gg_set_error("mock: out of memory"); return GG_ERR_NOMEM; }
 	r->pages = rows;
-	r->nblocks = (nrows * (uint64_t) (1 + ncols) * 8 + GG_BLCKSZ - 1) / GG_BLCKSZ;
+	{
+		/* the device's view (gg_abi.cu): 32 KB chunks of whole rows, an even number of them each */
+		const uint64_t per_chunk = (GG_BLCKSZ / (8ull * (1 + ncols))) & ~1ull;
+		r->nblocks = (nrows + per_chunk - 1) / per_chunk;
+	}
 	*out = r;
 	return GG_OK;
 }
 
 int gg_relation_read(gg_relation *r, uint64_t first_block, void *host_pages, uint64_t nblocks)
 {
+	if (nblocks > r->nblocks || first_block > r->nblocks - nblocks) { gg_set_error("mock: read outside the relation"); return GG_ERR_ARG; }
 	memcpy(host_pages, r->pages + first_block * GG_BLCKSZ, (size_t) nblocks * GG_BLCKSZ);
 	return GG_OK;
 }
